@@ -141,10 +141,10 @@ int variant_forward_tc(pb_variant_net *N, const int8_t *d_images, int64_t B, flo
             L.lo_h = layer == 0 ? (T.lo_mask & 1) : ((T.lo_mask >> 2) & 1);
             static bool attr_set = false;
             if (!attr_set) {
-                PB_CUDA(cudaFuncSetAttribute(tc::k_lstm_layer, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::PSMEM_BYTES));
+                PB_CUDA(cudaFuncSetAttribute(tc::k_lstm_layer, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::LSTM_SMEM_BYTES));
                 attr_set = true;
             }
-            tc::k_lstm_layer<<<(unsigned) (2 * Mt), tc::PG_THREADS, tc::PSMEM_BYTES, st>>>(L);
+            tc::k_lstm_layer<<<(unsigned) (2 * Mt), tc::LSTM_THREADS, tc::LSTM_SMEM_BYTES, st>>>(L);
             N->launches++;
             continue;
         }

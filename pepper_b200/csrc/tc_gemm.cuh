@@ -47,6 +47,11 @@ constexpr int PSTAGE_BYTES = 2 * TILE_BYTES + 2 * WTILE_BYTES;   // A_hi, A_lo, 
 constexpr int PSMEM_BYTES = PSTAGES * PSTAGE_BYTES + 256;         // 192 KB ring + barriers: one CTA per SM
 constexpr int CONS_WARPS = 8;                        // warps 0-7: two consumer warpgroups (rows 0-63, 64-127)
 constexpr int PG_THREADS = 32 * CONS_WARPS + 32;     // + warp 8: producer
+// k_lstm_layer: warps 8-11 form a producer warpgroup, so that setmaxnreg can move its registers to the consumers (one
+// thread issues the copies); the direction's 1,024 bias floats sit behind the ring and the barriers
+constexpr int LSTM_THREADS = 32 * CONS_WARPS + 128;
+constexpr int LSTM_SMEM_BYTES = PSMEM_BYTES + 1024 * 4;
+constexpr int LSTM_PROD_REGS = 40, LSTM_CONS_REGS = 232;   // 128 x 40 + 256 x 232 = 384 x 168, the launch's register file
 
 enum { EPI_BIAS = 0, EPI_SELU = 1, EPI_LSTM = 2 };
 
@@ -106,6 +111,11 @@ __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.alig
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// per-warpgroup register budget (every warp of the warpgroup executes it)
+template <int N>
+__device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // d[64 x 256] += A[64 x 16] B[256 x 16]^T, both operands K-major in shared memory (descriptors), fp32 accumulate
 __device__ __forceinline__ void wgmma_256(float (&d)[128], uint64_t adesc, uint64_t bdesc) {
@@ -341,6 +351,9 @@ __global__ void __launch_bounds__(PG_THREADS, 1) k_tc_gemm_p(Args G, int n_mt, i
 // The x-part of step t+1 (1 k-tile for the encoder layer, 16 for the decoder layer) does not depend on h_t and is
 // streamed while the last epilogue of step t runs.  One chunk of 8,448 candidates = 66 row tiles x 2 directions = 132
 // CTAs = one per H100 SM; the per-step kernel above stays as the cross-check path.
+// The epilogue touches no global load: each consumer lane loads the 32 cell states of its (row, unit) cells of a gate tile
+// before that tile's k-loop, so they arrive under the MMA (a lane owns the same cells at every step: its own store of step
+// t-1 precedes the load in program order), and the bias is staged in shared memory once per launch.
 struct LstmLayer {
     const op_t *x_hi, *x_lo;           // input sequence operand: tile (mt, t, kt) at mt * x_mt_stride + (t * x_nkt + kt) * TILE_ELEMS
     int64_t x_mt_stride;
@@ -357,9 +370,10 @@ struct LstmLayer {
     int lo_x, lo_h;                    // 1: the a_lo x w_hi product of the x-part / h-part is executed (0: two products)
 };
 
-__global__ void __launch_bounds__(PG_THREADS, 1) k_lstm_layer(LstmLayer G) {
+__global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
     extern __shared__ __align__(128) uint8_t smem[];
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem + PSTAGES * PSTAGE_BYTES);
+    float *sbias = reinterpret_cast<float *>(smem + PSMEM_BYTES);
     const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + PSTAGES), bar_h = smem_u32(bars + 2 * PSTAGES);
     const uint32_t smem_base = smem_u32(smem);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -371,10 +385,12 @@ __global__ void __launch_bounds__(PG_THREADS, 1) k_lstm_layer(LstmLayer G) {
         mbar_init(bar_h, CONS_WARPS);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
+    for (int i = threadIdx.x; i < 4 * PBN; i += LSTM_THREADS) sbias[i] = G.bias[dir][i];
     __syncthreads();
 
-    if (warp == CONS_WARPS) {
-        if (lane == 0) {
+    if (warp >= CONS_WARPS) {
+        reg_dealloc<LSTM_PROD_REGS>();
+        if (threadIdx.x == 32 * CONS_WARPS) {
             uint32_t g = 0;
             for (int t = 0; t < G.T; t++) {
                 const int tt = dir ? G.T - 1 - t : t, tp = dir ? tt + 1 : tt - 1;
@@ -403,12 +419,12 @@ __global__ void __launch_bounds__(PG_THREADS, 1) k_lstm_layer(LstmLayer G) {
         }
         return;
     }
+    reg_alloc<LSTM_CONS_REGS>();
     const int wg = warp >> 2, q = lane & 3;
     const int r128 = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * (q & 1);      // row of this lane's cells
     const int row = mt * BM + r128;
     const bool valid = row < G.M;
     float *cst = G.c[dir];
-    const float *bias = G.bias[dir];
     const bool lo_x = G.x_lo != nullptr && G.lo_x != 0, lo_h = G.lo_h != 0;
     uint32_t g = 0;
     float acc[128];
@@ -417,15 +433,19 @@ __global__ void __launch_bounds__(PG_THREADS, 1) k_lstm_layer(LstmLayer G) {
         const int y_kt0 = tt * 16 + dir * 8;
         const int nkt = G.x_nkt + (t > 0 ? 8 : 0);
         for (int nt = 0; nt < 4; nt++) {
+            // cell states of units nt * 64 + 2 i + q / 2, in flight during the k-loop
+            float *cp = cst + (int64_t) (nt * (PBN / 4) + (q >> 1)) * G.c_ld + row;
+            float c_prev[PBN / 8];
+#pragma unroll
+            for (int i = 0; i < PBN / 8; i++) c_prev[i] = valid ? __ldcg(cp + (int64_t) (2 * i) * G.c_ld) : 0.f;
             mma_tile(acc, smem_base, bar_full, bar_empty, g, nkt, G.x_nkt, lo_x, lo_h, wg, lane);
 #pragma unroll
             for (int i = 0; i < PBN / 8; i++) {
                 const int j = nt * (PBN / 4) + 2 * i + (q >> 1);
                 float gt[4];
-                gates4(acc, i, __ldg(reinterpret_cast<const float2 *>(bias + nt * PBN + 8 * i + 2 * q)), q, gt);
-                float *cp = cst + (int64_t) j * G.c_ld + row;
-                const float cn = sigm(gt[1]) * (valid ? *cp : 0.f) + sigm(gt[0]) * tanh_fast(gt[2]);
-                if (valid) *cp = cn;
+                gates4(acc, i, *reinterpret_cast<const float2 *>(sbias + nt * PBN + 8 * i + 2 * q), q, gt);
+                const float cn = sigm(gt[1]) * c_prev[i] + sigm(gt[0]) * tanh_fast(gt[2]);
+                if (valid) cp[(int64_t) (2 * i) * G.c_ld] = cn;
                 const float hn = sigm(gt[3]) * tanh_fast(cn);
                 const int64_t o = (int64_t) mt * G.y_mt_stride + (int64_t) y_kt0 * TILE_ELEMS + tile_off(j, r128);
                 store_h(hn, valid && !(q & 2), G.y_hi, G.y_lo, o,
