@@ -33,11 +33,14 @@ typedef __nv_bfloat16 op_t;
 #define OP_PTX "bf16"
 __host__ __device__ __forceinline__ uint16_t op_bits(float v) { return __bfloat16_as_ushort(__float2bfloat16_rn(v)); }
 __host__ __device__ __forceinline__ float op_val(uint32_t b) { return __bfloat162float(__ushort_as_bfloat16((unsigned short) (b & 0xffffu))); }
+__device__ __forceinline__ uint16_t op_bits_unit(float v) { return op_bits(v); }
 #else
 typedef __half op_t;
 #define OP_PTX "f16"
 __host__ __device__ __forceinline__ uint16_t op_bits(float v) { return __half_as_ushort(__float2half_rn(fminf(fmaxf(v, -65504.f), 65504.f))); }
 __host__ __device__ __forceinline__ float op_val(uint32_t b) { return __half2float(__ushort_as_half((unsigned short) (b & 0xffffu))); }
+// op_bits of a value with |v| <= 1 (LSTM hidden states), where the clamp is the identity
+__device__ __forceinline__ uint16_t op_bits_unit(float v) { return __half_as_ushort(__float2half_rn(v)); }
 #endif
 
 constexpr int BM = 128, BK = 32;
@@ -148,20 +151,29 @@ __device__ __forceinline__ void wgmma_256(float (&d)[128], uint64_t adesc, uint6
         : "l"(adesc), "l"(bdesc), "r"(1));
 }
 
-// exp via ex2.approx (2 ulp) + fast divide: absolute error ~1e-6, far inside the 1e-3 parity tolerance
-__device__ __forceinline__ float sigm(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
+// exp via ex2.approx (2 ulp) + fast divide: absolute error ~1e-6, far inside the 1e-3 parity tolerance.  exp_ftz is __expf
+// without its fix-up for results below 2^-126 (flushed to zero instead): the bits differ only where 1 + e rounds to 1
+// either way (sigm), and never occur in tanh_fast (e >= e^-30).
+__device__ __forceinline__ float exp_ftz(float x) {
+    float y;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x * 1.4426950408889634f));
+    return y;
+}
+__device__ __forceinline__ float sigm(float x) { return __fdividef(1.0f, 1.0f + exp_ftz(-x)); }
 __device__ __forceinline__ float tanh_fast(float x) {
-    const float e = __expf(2.0f * fminf(fmaxf(x, -15.0f), 15.0f));
+    const float e = exp_ftz(2.0f * fminf(fmaxf(x, -15.0f), 15.0f));
     return 1.0f - __fdividef(2.0f, e + 1.0f);
 }
 __device__ __forceinline__ float selu(float x) {
     const float alpha = 1.6732632423543772848170429916717f, scale = 1.0507009873554804934193349852946f;
     return x > 0.f ? scale * x : scale * alpha * (__expf(x) - 1.0f);
 }
-// 2 fp32 -> 2 hi + 2 lo 16-bit operands, 4 B each
+// 2 fp32 -> 2 hi + 2 lo 16-bit operands, 4 B each.  UNIT: |a|, |b| <= 1, no range clamp needed (same bits)
+template <bool UNIT = false>
 __device__ __forceinline__ void split2(float a, float b, uint32_t &hi, uint32_t &lo) {
-    const uint16_t h0 = op_bits(a), h1 = op_bits(b);
-    const uint16_t l0 = op_bits(a - op_val(h0)), l1 = op_bits(b - op_val(h1));
+    const uint16_t h0 = UNIT ? op_bits_unit(a) : op_bits(a), h1 = UNIT ? op_bits_unit(b) : op_bits(b);
+    const uint16_t l0 = UNIT ? op_bits_unit(a - op_val(h0)) : op_bits(a - op_val(h0));
+    const uint16_t l1 = UNIT ? op_bits_unit(b - op_val(h1)) : op_bits(b - op_val(h1));
     hi = (uint32_t) h0 | ((uint32_t) h1 << 16);
     lo = (uint32_t) l0 | ((uint32_t) l1 << 16);
 }
@@ -240,15 +252,15 @@ __device__ __forceinline__ void gates4(const float (&acc)[128], int i, float2 bz
     gt[2] = odd ? b0 : r0; gt[3] = odd ? b1 : r1;
 }
 // h of units (2i, 2i + 1) meet in lanes q and q ^ 2: the even-unit lane stores both (4 B operand words, 8 B fp32 pair)
+template <bool UNIT = false>
 __device__ __forceinline__ void store_h(float hn, bool store, op_t *y_hi, op_t *y_lo, int64_t o, float *y_f32) {
     uint32_t hi, lo;
     const float hn1 = __shfl_xor_sync(0xffffffffu, hn, 2);
-    split2(hn, hn1, hi, lo);
-    if (store) {
-        *reinterpret_cast<uint32_t *>(y_hi + o) = hi;
-        *reinterpret_cast<uint32_t *>(y_lo + o) = lo;
-        if (y_f32) *reinterpret_cast<float2 *>(y_f32) = make_float2(hn, hn1);
-    }
+    split2<UNIT>(hn, hn1, hi, lo);
+    // predicated stores, no branch: a branch per cell would keep the scheduler from overlapping consecutive cells
+    if (store) *reinterpret_cast<uint32_t *>(y_hi + o) = hi;
+    if (store) *reinterpret_cast<uint32_t *>(y_lo + o) = lo;
+    if (store && y_f32) *reinterpret_cast<float2 *>(y_f32) = make_float2(hn, hn1);
 }
 __device__ __forceinline__ float load_h(const op_t *hi, const op_t *lo, int64_t o) {
     return op_val(reinterpret_cast<const uint16_t *>(hi)[o]) + op_val(reinterpret_cast<const uint16_t *>(lo)[o]);
@@ -357,6 +369,7 @@ __global__ void __launch_bounds__(PG_THREADS, 1) k_tc_gemm_p(Args G, int n_mt, i
 // The x-part of step t+1 (1 k-tile for the encoder layer, 16 for the decoder layer) does not depend on h_t and is
 // streamed while the last epilogue of step t runs.  One chunk of 8,448 candidates = 66 row tiles x 2 directions = 132
 // CTAs = one per H100 SM; the per-step kernel above stays as the cross-check path.
+// Both consumer warpgroups (64 rows each) multiply a 256-column gate tile together, then both run its epilogue.
 // The epilogue touches no global load: each consumer lane loads the 32 cell states of its (row, unit) cells of a gate tile
 // before that tile's k-loop, so they arrive under the MMA (a lane owns the same cells at every step: its own store of step
 // t-1 precedes the load in program order), and the bias is staged in shared memory once per launch.
@@ -431,33 +444,40 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
     const int r128 = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * (q & 1);      // row of this lane's cells
     const int row = mt * BM + r128;
     const bool valid = row < G.M;
-    float *cst = G.c[dir];
     const bool lo_x = G.x_lo != nullptr && G.lo_x != 0, lo_h = G.lo_h != 0;
     const float inv_s = G.inv_scale[dir];
+    const int c2 = 2 * (int) G.c_ld;                                  // cell state of unit j + 2 lies c2 floats after unit j
     uint32_t g = 0;
     float acc[128];
     for (int t = 0; t < G.T; t++) {
         const int tt = dir ? G.T - 1 - t : t;
-        const int y_kt0 = tt * 16 + dir * 8;
         const int nkt = G.x_nkt + (t > 0 ? 8 : 0);
+        const int64_t y0 = (int64_t) mt * G.y_mt_stride + (int64_t) (tt * 16 + dir * 8) * TILE_ELEMS + r128 * 8;
         for (int nt = 0; nt < 4; nt++) {
             // cell states of units nt * 64 + 2 i + q / 2, in flight during the k-loop
-            float *cp = cst + (int64_t) (nt * (PBN / 4) + (q >> 1)) * G.c_ld + row;
+            float *cp = G.c[dir] + (int64_t) (nt * (PBN / 4) + (q >> 1)) * G.c_ld + row;
             float c_prev[PBN / 8];
 #pragma unroll
-            for (int i = 0; i < PBN / 8; i++) c_prev[i] = valid ? __ldcg(cp + (int64_t) (2 * i) * G.c_ld) : 0.f;
+            for (int i = 0; i < PBN / 8; i++) c_prev[i] = valid ? __ldcg(cp + i * c2) : 0.f;
             mma_tile(acc, smem_base, bar_full, bar_empty, g, nkt, G.x_nkt, lo_x, lo_h, wg, lane);
+            // the stores recompute their addresses (IMAD per cell) instead of keeping the 32 load pointers alive across
+            // the k-loop
+            int c2s;
+            asm volatile("mov.b32 %0, %1;" : "=r"(c2s) : "r"(c2));
+            const float *sb = sbias + nt * PBN + 2 * q;
+            // units nt * 64 .. + 63 are operand k-tiles 2 nt, 2 nt + 1 of this step
+            op_t *yh = G.y_hi + y0 + 2 * nt * TILE_ELEMS, *yl = G.y_lo + y0 + 2 * nt * TILE_ELEMS;
+            float *yf = G.y_f32 ? G.y_f32 + (int64_t) row * G.ldy + (int64_t) tt * 512 + dir * 256 + nt * (PBN / 4) + (q >> 1) : nullptr;
 #pragma unroll
             for (int i = 0; i < PBN / 8; i++) {
-                const int j = nt * (PBN / 4) + 2 * i + (q >> 1);
                 float gt[4];
-                gates4(acc, i, *reinterpret_cast<const float2 *>(sbias + nt * PBN + 8 * i + 2 * q), inv_s, q, gt);
+                gates4(acc, i, *reinterpret_cast<const float2 *>(sb + 8 * i), inv_s, q, gt);
                 const float cn = sigm(gt[1]) * c_prev[i] + sigm(gt[0]) * tanh_fast(gt[2]);
-                if (valid) cp[(int64_t) (2 * i) * G.c_ld] = cn;
                 const float hn = sigm(gt[3]) * tanh_fast(cn);
-                const int64_t o = (int64_t) mt * G.y_mt_stride + (int64_t) y_kt0 * TILE_ELEMS + tile_off(j, r128);
-                store_h(hn, valid && !(q & 2), G.y_hi, G.y_lo, o,
-                        G.y_f32 ? G.y_f32 + (int64_t) row * G.ldy + (int64_t) tt * 512 + dir * 256 + j : nullptr);
+                if (valid) cp[i * c2s] = cn;
+                // element (unit nt * 64 + 2 i, row r128) of the step's operand tiles, relative to the lane's base
+                store_h<true>(hn, valid && !(q & 2), yh, yl, (i >> 4) * TILE_ELEMS + ((i & 15) >> 2) * 1024 + 2 * (i & 3),
+                              yf ? yf + 2 * i : nullptr);
             }
         }
         // h_t of this warp's rows is complete (all four gate tiles): publish it to the producer thread
