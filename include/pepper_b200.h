@@ -220,6 +220,10 @@ int pb_bam_inflate_split(pb_bam_t *bam, int64_t *host_blocks, int64_t *device_bl
 /* diagnostics: raw DEFLATE streams inflated by the GPU kernel (outputs concatenated; h_status[i] != 0 = rejected stream) */
 int pb_inflate_blocks_host(const uint8_t *h_comp, int64_t comp_bytes, const int64_t *h_in_off, const int32_t *h_in_len,
                            const int32_t *h_out_len, int64_t n_blocks, uint8_t *h_out, int32_t *h_status, void *stream);
+/* diagnostics: pb_inflate_blocks_host with the symbol decoder chosen per call instead of by PB_INFLATE_SPEC: spec 1 = the
+ * warp-parallel speculative decode, 0 = the one-decoder-per-warp loop */
+int pb_test_inflate_blocks(const uint8_t *h_comp, int64_t comp_bytes, const int64_t *h_in_off, const int32_t *h_in_len,
+                           const int32_t *h_out_len, int64_t n_blocks, uint8_t *h_out, int32_t *h_status, void *stream, int spec);
 
 typedef struct pb_fasta pb_fasta_t;
 int pb_fasta_open(pb_fasta_t **out, const char *path);          /* FASTA_handler(path): path + ".fai" must exist       */

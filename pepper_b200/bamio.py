@@ -31,6 +31,7 @@ def _bind(L):
     L.pb_bam_set_host_share.argtypes = [C.c_void_p, C.c_double]
     L.pb_bam_inflate_split.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.pb_inflate_blocks_host.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.pb_test_inflate_blocks.argtypes = L.pb_inflate_blocks_host.argtypes + [C.c_int]
     L.pb_fasta_open.argtypes = [C.POINTER(C.c_void_p), C.c_char_p]
     L.pb_fasta_close.argtypes = [C.c_void_p]
     L.pb_fasta_n_contigs.argtypes = [C.c_void_p]
@@ -103,20 +104,29 @@ class DeviceRecordsView:
                            arr(s.seq, (nb + 1) // 2, np.uint8), arr(s.qual, nb, np.uint8), arr(s.cigar, nc, np.uint32))
 
 
-def inflate_blocks(streams: list[bytes], sizes: list[int]):
-    """Raw DEFLATE streams through the GPU kernel (diagnostics / tests): returns (list of outputs, status array)."""
+def inflate_blocks(streams: list[bytes], sizes: list[int], in_lens: list[int] | None = None, spec: int | None = None):
+    """Raw DEFLATE streams through the GPU kernel (diagnostics / tests): returns (list of outputs, status array).
+    The streams lie back to back in one buffer; `in_lens` (default: each stream's length) is the payload length the kernel is
+    given for each, so a shorter one leaves the stream's remaining bytes in memory right after the payload.  `spec` 1 / 0
+    selects the speculative / one-decoder symbol loop (pb_test_inflate_blocks); None leaves it to PB_INFLATE_SPEC."""
     _lib.require_gpu()
     L = _lib.lib()
     _bind(L)
     n = len(streams)
-    comp = np.frombuffer(b"".join(streams) + b"\0" * 16, dtype=np.uint8).copy()
-    lens = np.array([len(s) for s in streams], dtype=np.int32)
-    offs = np.concatenate([[0], np.cumsum(lens[:-1])]).astype(np.int64) if n else np.zeros(0, np.int64)
+    comp = np.frombuffer(b"".join(streams) + b"\0" * 64, dtype=np.uint8).copy()
+    full = np.array([len(s) for s in streams], dtype=np.int64)
+    offs = np.concatenate([[0], np.cumsum(full[:-1])]).astype(np.int64) if n else np.zeros(0, np.int64)
+    lens = np.array(full if in_lens is None else in_lens, dtype=np.int32)
+    assert lens.shape == (n,) and np.all((lens >= 0) & (lens <= full))
     outl = np.array(sizes, dtype=np.int32)
     out = np.zeros(int(outl.sum()) + 1, dtype=np.uint8)
     status = np.zeros(max(n, 1), dtype=np.int32)
-    _lib.check(L.pb_inflate_blocks_host(comp.ctypes.data, int(lens.sum()), offs.ctypes.data, lens.ctypes.data, outl.ctypes.data, n,
-                                        out.ctypes.data, status.ctypes.data, None), "pb_inflate_blocks_host")
+    args = (comp.ctypes.data, int(full.sum()), offs.ctypes.data, lens.ctypes.data, outl.ctypes.data, n, out.ctypes.data,
+            status.ctypes.data, None)
+    if spec is None:
+        _lib.check(L.pb_inflate_blocks_host(*args), "pb_inflate_blocks_host")
+    else:
+        _lib.check(L.pb_test_inflate_blocks(*args, int(spec)), "pb_test_inflate_blocks")
     cuts = np.concatenate([[0], np.cumsum(outl)]).astype(np.int64)
     return [bytes(out[cuts[i]:cuts[i + 1]]) for i in range(n)], status[:n]
 

@@ -912,9 +912,10 @@ extern "C" int pb_bam_inflate_split(pb_bam_t *b, int64_t *host_blocks, int64_t *
 }
 
 // diagnostics / tests: inflate `n_blocks` raw DEFLATE streams on the GPU (h_in_off / h_in_len / h_out_len per stream, outputs
-// concatenated in order); h_status[i] != 0 marks a stream the kernel rejected
-extern "C" int pb_inflate_blocks_host(const uint8_t *h_comp, int64_t comp_bytes, const int64_t *h_in_off, const int32_t *h_in_len, const int32_t *h_out_len,
-                                      int64_t n_blocks, uint8_t *h_out, int32_t *h_status, void *stream_) {
+// concatenated in order); h_status[i] != 0 marks a stream the kernel rejected.  spec: 1 / 0 = the speculative / one-decoder
+// symbol loop, -1 = whichever launch_inflate picks
+static int inflate_blocks_host(const uint8_t *h_comp, int64_t comp_bytes, const int64_t *h_in_off, const int32_t *h_in_len, const int32_t *h_out_len,
+                               int64_t n_blocks, uint8_t *h_out, int32_t *h_status, void *stream_, int spec) {
     using namespace pb::bgzf;
     if (!h_comp || !h_in_off || !h_in_len || !h_out_len || !h_out || !h_status) { set_error("null argument"); return PB_ERR_ARG; }
     int ndev = 0;
@@ -934,13 +935,28 @@ extern "C" int pb_inflate_blocks_host(const uint8_t *h_comp, int64_t comp_bytes,
         if ((rc = upload(db, desc.data(), sizeof(BlockDesc) * n_blocks, st)) != PB_OK) break;
         if ((rc = ds.reserve(sizeof(int) * (n_blocks + 1))) != PB_OK) break;
         if ((rc = du.reserve((size_t) utotal + 64)) != PB_OK) break;
-        if (n_blocks && (rc = launch_inflate(dc.as<uint8_t>(), db.as<BlockDesc>(), n_blocks, du.as<uint8_t>(), ds.as<int>(), st)) != PB_OK) break;
+        if (n_blocks && spec < 0 && (rc = launch_inflate(dc.as<uint8_t>(), db.as<BlockDesc>(), n_blocks, du.as<uint8_t>(), ds.as<int>(), st)) != PB_OK) break;
+        if (n_blocks && spec >= 0) {
+            const unsigned grid = (unsigned) ceil_div(n_blocks, WARPS_PER_CTA);
+            if (spec) k_bgzf_inflate<true><<<grid, 32 * WARPS_PER_CTA, 0, st>>>(dc.as<uint8_t>(), db.as<BlockDesc>(), (int) n_blocks, du.as<uint8_t>(), ds.as<int>());
+            else k_bgzf_inflate<false><<<grid, 32 * WARPS_PER_CTA, 0, st>>>(dc.as<uint8_t>(), db.as<BlockDesc>(), (int) n_blocks, du.as<uint8_t>(), ds.as<int>());
+            if (cudaGetLastError() != cudaSuccess) { set_error("inflate launch failed"); rc = PB_ERR_CUDA; break; }
+        }
         cudaMemcpyAsync(h_status, ds.p, sizeof(int) * n_blocks, cudaMemcpyDeviceToHost, st);
         if (utotal) cudaMemcpyAsync(h_out, du.p, (size_t) utotal, cudaMemcpyDeviceToHost, st);
         if (cudaStreamSynchronize(st) != cudaSuccess) { set_error("inflate kernel failed: %s", cudaGetErrorString(cudaGetLastError())); rc = PB_ERR_CUDA; }
     } while (0);
     dc.release(); db.release(); ds.release(); du.release();
     return rc;
+}
+extern "C" int pb_inflate_blocks_host(const uint8_t *h_comp, int64_t comp_bytes, const int64_t *h_in_off, const int32_t *h_in_len, const int32_t *h_out_len,
+                                      int64_t n_blocks, uint8_t *h_out, int32_t *h_status, void *stream) {
+    return inflate_blocks_host(h_comp, comp_bytes, h_in_off, h_in_len, h_out_len, n_blocks, h_out, h_status, stream, -1);
+}
+extern "C" int pb_test_inflate_blocks(const uint8_t *h_comp, int64_t comp_bytes, const int64_t *h_in_off, const int32_t *h_in_len, const int32_t *h_out_len,
+                                      int64_t n_blocks, uint8_t *h_out, int32_t *h_status, void *stream, int spec) {
+    if (spec != 0 && spec != 1) { set_error("pb_test_inflate_blocks: spec must be 0 or 1"); return PB_ERR_ARG; }
+    return inflate_blocks_host(h_comp, comp_bytes, h_in_off, h_in_len, h_out_len, n_blocks, h_out, h_status, stream, spec);
 }
 
 // ----------------------------------------------------------------------------------------------------------- FASTA

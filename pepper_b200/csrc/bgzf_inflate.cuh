@@ -79,8 +79,11 @@ struct BitReader {
 };
 
 // Builds the primary table + the canonical (count, sorted symbols) arrays for `n` symbols with code lengths lens[0..n).
-// Whole warp; returns false when the lengths over-subscribe the code space.
-__device__ bool build_table(const uint8_t *lens, int n, uint16_t *tab, int tab_bits, uint16_t *cnt, uint16_t *sorted, uint16_t *code, int lane) {
+// Whole warp; returns false when the lengths over-subscribe the code space, and when they leave part of it unused unless
+// `lenient` and no code is longer than 1 bit (zlib's inflate_table: a literal/length or distance set may be one 1-bit code
+// or empty; a code-length set must be complete).
+__device__ bool build_table(const uint8_t *lens, int n, uint16_t *tab, int tab_bits, uint16_t *cnt, uint16_t *sorted, uint16_t *code, bool lenient,
+                            int lane) {
     if (lane < 16) cnt[lane] = 0;
     for (int i = lane; i < (1 << tab_bits); i += 32) tab[i] = 0;
     __syncwarp();
@@ -88,8 +91,9 @@ __device__ bool build_table(const uint8_t *lens, int n, uint16_t *tab, int tab_b
     if (lane == 0) {
         for (int s = 0; s < n; s++) cnt[lens[s]]++;
         cnt[0] = 0;
-        int left = 1;
-        for (int l = 1; l <= 15; l++) { left = (left << 1) - cnt[l]; if (left < 0) ok = false; }
+        int left = 1, longest = 0;
+        for (int l = 1; l <= 15; l++) { left = (left << 1) - cnt[l]; if (left < 0) ok = false; if (cnt[l]) longest = l; }
+        if (left > 0 && !(lenient && longest <= 1)) ok = false;
         // canonical codes + symbols sorted by (length, symbol)
         uint16_t next[16], offs[16];
         uint32_t c = 0;
@@ -220,7 +224,7 @@ __device__ int spec_symbols(const uint8_t *payload, int64_t in_bits, int64_t &bp
         }
         if (err) return err;
         if (pos + off > out_len) return 4;
-        if (bp + p > in_bits + 64) return 7;                                     // ran past the payload (tolerates the padded tail of the last code)
+        if (bp + p > in_bits) return 7;                                          // a symbol ends past the payload (BitReader::overrun)
         // ---- output: literals and short matches that read only bytes of earlier rounds are written by their own lanes
         const bool mine = myoff >= 0;
         bool coop = false;
@@ -301,7 +305,7 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA) k_bgzf_inflate(const uint8
         int hlit = 288, hdist = 30;
         if (type == 1) {
             for (int s = lane; s < 288; s += 32) T.lens[s] = s < 144 ? 8 : s < 256 ? 9 : s < 280 ? 7 : 8;
-            if (lane < 30) T.lens[288 + lane] = 5;
+            T.lens[288 + lane] = 5;                                     // distances 30 / 31 complete the code; decoding them is an error
             __syncwarp();
         } else {
             // dynamic: HLIT, HDIST, HCLEN, the code-length code, then the literal/length + distance code lengths
@@ -313,7 +317,7 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA) k_bgzf_inflate(const uint8
             __syncwarp();
             if (lane == 0) for (int i = 0; i < hclen; i++) T.lens[c_clen_order[i]] = (uint8_t) br.get(3);
             __syncwarp();
-            if (!build_table(T.lens, 19, T.dist, 7, T.dist_cnt, T.dist_sym, T.code, lane)) { err = 2; break; }
+            if (!build_table(T.lens, 19, T.dist, 7, T.dist_cnt, T.dist_sym, T.code, false, lane)) { err = 2; break; }
             if (lane == 0) {
                 uint8_t tmp[320];
                 int i = 0;
@@ -341,9 +345,8 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA) k_bgzf_inflate(const uint8
             if (err) break;
             __syncwarp();
         }
-        if (!build_table(T.lens, 288, T.lit, LIT_BITS, T.lit_cnt, T.lit_sym, T.code, lane)) { err = 2; break; }
-        // an incomplete distance code is legal when only one distance code is used (zlib emits it): do not reject under-subscription
-        if (!build_table(T.lens + 288, 30, T.dist, DIST_BITS, T.dist_cnt, T.dist_sym, T.code, lane)) { err = 2; break; }
+        if (!build_table(T.lens, 288, T.lit, LIT_BITS, T.lit_cnt, T.lit_sym, T.code, true, lane)) { err = 2; break; }
+        if (!build_table(T.lens + 288, 32, T.dist, DIST_BITS, T.dist_cnt, T.dist_sym, T.code, true, lane)) { err = 2; break; }
         if (SPEC) {
             // ---- warp-parallel speculative decode (above); lane 0's bit reader is re-synchronised at the end-of-block position
             int64_t bp = 0;

@@ -29,9 +29,13 @@ def reg2bin(beg: int, end: int) -> int:
     return 0
 
 
-def _bgzf_block(payload: bytes, level: int) -> bytes:
-    co = zlib.compressobj(level, zlib.DEFLATED, -15)
-    data = co.compress(payload) + co.flush()
+def _bgzf_block(payload: bytes, level: int, deflate=None) -> bytes:
+    """One BGZF member; `deflate(payload)` -> raw DEFLATE bytes replaces zlib at `level` when given."""
+    if deflate is None:
+        co = zlib.compressobj(level, zlib.DEFLATED, -15)
+        data = co.compress(payload) + co.flush()
+    else:
+        data = deflate(payload)
     bsize = 18 + len(data) + 8
     assert bsize <= 65536
     return (b"\x1f\x8b\x08\x04" + b"\0\0\0\0" + b"\0\xff" + struct.pack("<H", 6) + b"BC" + struct.pack("<HH", 2, bsize - 1)
@@ -44,10 +48,14 @@ def record_ref_len(cigar_words: np.ndarray) -> int:
 
 
 def write_bam(path: str, contigs: list[tuple[str, int]], batches: dict[int, RecordBatch], header_text: str | None = None,
-              block_payload: int = 60000, level: int = 1, long_cigar_over: int = 65535, aux: bytes = b"") -> None:
+              block_payload: int = 60000, level: int = 1, long_cigar_over: int = 65535, aux=b"", cg_first: bool = False,
+              deflate=None) -> None:
     """`batches`: tid -> coordinate-sorted RecordBatch.  Writes `path` and `path + '.bai'`.  Records are cut into BGZF
     blocks every `block_payload` bytes regardless of record boundaries (records span blocks, as in real files).  CIGARs
-    with more than `long_cigar_over` ops use the CG:B,I convention (SAMv1 4.2.2)."""
+    with more than `long_cigar_over` ops use the CG:B,I convention (SAMv1 4.2.2).  `aux`: the encoded aux tags of every
+    record, or a function of the record's index in its batch that returns them; the CG tag goes after them, or before them
+    with `cg_first`.  `deflate`: payload bytes -> raw DEFLATE stream of each BGZF block (default zlib at `level`); the
+    index holds the virtual offsets of the blocks as written."""
     if header_text is None:
         header_text = "@HD\tVN:1.6\tSO:coordinate\n" + "".join(f"@SQ\tSN:{n}\tLN:{l}\n" for n, l in contigs) + \
             "@RG\tID:rg1\tSM:sample_b200\n"
@@ -73,11 +81,12 @@ def write_bam(path: str, contigs: list[tuple[str, int]], batches: dict[int, Reco
                 codes = np.concatenate([codes, np.zeros(1, np.uint8)])
             seq = ((codes[0::2] << 4) | codes[1::2]).astype(np.uint8).tobytes()
             qual = b.qual[so:se].tobytes()
-            tags = aux
+            tags = aux(r) if callable(aux) else aux
             cig_field = cig
             if cig.shape[0] > long_cigar_over:
                 cig_field = np.array([(l_seq << 4) | 4, (rlen << 4) | 3], dtype="<u4")
-                tags = tags + b"CGBI" + struct.pack("<i", cig.shape[0]) + cig.tobytes()
+                cg = b"CGBI" + struct.pack("<i", cig.shape[0]) + cig.tobytes()
+                tags = cg + tags if cg_first else tags + cg
             body = struct.pack("<iiBBHHHiiii", tid, pos, len(name), int(b.mapq[r]), reg2bin(pos, end), cig_field.shape[0],
                                int(b.flag[r]), l_seq, -1, -1, 0) + name + cig_field.tobytes() + seq + qual + tags
             rec = struct.pack("<i", len(body)) + body
@@ -90,7 +99,7 @@ def write_bam(path: str, contigs: list[tuple[str, int]], batches: dict[int, Reco
     ustart, coff, out = [], [], []
     c = 0
     for s in range(0, len(stream), block_payload):
-        blk = _bgzf_block(stream[s:s + block_payload], level)
+        blk = _bgzf_block(stream[s:s + block_payload], level, deflate)
         ustart.append(s)
         coff.append(c)
         out.append(blk)

@@ -18,6 +18,6 @@ for tool in memcheck racecheck; do
     run polish_encoder $tool tests/test_polish_encoder_gpu.py -k "kat"                                 # k_polish_count
     run nets_variant $tool "tests/test_nets_gpu.py::test_variant_net_vs_oracle[130-2-1]"                 # k_lstm_layer, k_tc_gemm_p
     run nets_polish $tool "tests/test_nets_gpu.py::test_polish_net_vs_oracle[5-5-1]"                     # k_gru_layer
-    run inflate $tool tests/test_inflate_gpu.py -k "inflate_matches or rejects"                         # k_bgzf_inflate
+    run inflate $tool tests/test_inflate_gpu.py tests/test_inflate_edges_gpu.py -k "inflate_matches or rejects or case_table or cut_short"   # k_bgzf_inflate
 done
 cat "$OUT/sanitizer_summary.txt"
