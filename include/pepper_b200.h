@@ -615,6 +615,64 @@ int pb_variant_find_candidates_host(const int64_t *h_positions, const int32_t *h
                                     const pb_candidate_options_t *opt,
                                     uint8_t *h_flags, uint8_t *h_genotype, void *stream);
 
+/* ------------------------------------------------------------------------
+ * VCF data lines on the GPU.  After the selection above, the records are grouped
+ * by (contig, position) and each site becomes one line, as in
+ * VCFWriter.candidate_list_to_variant + write_vcf_records (pepper_variant
+ * VcfWriter.py:48-218):
+ * - the selected records, first occurrence of each (ref, alt);
+ * - ranked by (genotype, genotype probability) descending, ties in arrival order;
+ * - the first allowed_multiallelics of them, alleles extended to the longest REF.
+ * Text: CHROM POS ID REF ALT QUAL FILTER INFO FORMAT SAMPLE, FORMAT
+ * GT:AP:GQ:DP:AD:VAF:REP, the bytes pysam writes.  AP is "%.6g" of the float32
+ * exactly; VAF comes from vaf_table.  Lines are in (contig id, position) order.
+ * The caller applies the writer's cross-contig rules (lexical contig order, the
+ * repeated-position skip of VcfWriter.py:151-152) with the line table.
+ * ---------------------------------------------------------------------- */
+typedef struct {
+    int32_t allowed_multiallelics;   /* 1..16 */
+    int32_t reserved;
+    double  snp_q_cutoff, indel_q_cutoff, snp_q_cutoff_in_lc, indel_q_cutoff_in_lc;
+} pb_vcf_options_t;
+#define PB_VCF_CLASS_PEPPER    0     /* PEPPER_VARIANT_OUTPUT_PEPPER */
+#define PB_VCF_CLASS_VC_SNP    1     /* PEPPER_VARIANT_OUTPUT_VARIANT_CALLING + _SNPs */
+#define PB_VCF_CLASS_VC_INDEL  2     /* PEPPER_VARIANT_OUTPUT_VARIANT_CALLING + _INDEL */
+typedef struct {
+    int64_t pos;          /* 0-based site position */
+    int64_t text_off;     /* byte offset of the line in the text */
+    int32_t contig;       /* contig id (index into the job's names) */
+    int32_t ref_len;      /* length of REF */
+    int32_t cls;          /* PB_VCF_CLASS_* */
+    int32_t text_len;     /* bytes of the line, '\n' included */
+} pb_vcf_line_t;
+/* device arrays: contig id per region id, contig names back to back with name_off [n_contigs + 1],
+ * vaf_table [256][256][8]: NUL-padded "%g" of round(ad / max(1, dp), 3) at [ad][dp] */
+typedef struct {
+    const int32_t *contig_of_region;
+    const char    *names;
+    const int64_t *name_off;
+    const char    *vaf_table;
+} pb_vcf_job_t;
+/* Every record of the columns (device) -> text (device, text_cap bytes) + line table (device, lines_cap).
+ * *n_text / *n_lines: the exact need.  PB_ERR_CAPACITY when d_text / d_lines is NULL or short (nothing written). */
+int pb_variant_vcf_device(const pb_candidate_columns_t *cols, const float *d_probs, int64_t n,
+                          const pb_region_t *d_regions, const char *d_ref, const pb_vcf_job_t *job,
+                          const pb_candidate_options_t *sel_opt, const pb_vcf_options_t *vcf_opt,
+                          char *d_text, int64_t text_cap, pb_vcf_line_t *d_lines, int64_t lines_cap,
+                          int64_t *n_text, int64_t *n_lines, void *stream);
+/* the same over host arrays; h_names holds name_off[n_contigs] bytes */
+int pb_variant_vcf_host(const int64_t *h_positions, const int32_t *h_region_of, const uint8_t *h_depths,
+                        const uint8_t *h_freqs, const char *h_keys, const float *h_probs, int64_t n,
+                        const pb_region_t *h_regions, int64_t n_regions, const char *h_ref, int64_t ref_bytes,
+                        const int32_t *h_contig_of_region, const char *h_names, const int64_t *h_name_off,
+                        int64_t n_contigs, const char *h_vaf_table, const pb_candidate_options_t *sel_opt,
+                        const pb_vcf_options_t *vcf_opt, char *h_text, int64_t text_cap, pb_vcf_line_t *h_lines,
+                        int64_t lines_cap, int64_t *n_text, int64_t *n_lines, void *stream);
+/* diagnostics: h_out [n][16] NUL-padded, the device's "%.6g" of each float32 */
+int pb_test_format_g(const float *h_x, int64_t n, char *h_out);
+/* diagnostics: h_qual [n], the device's QUAL = max(1, int(-10 log10(max(1e-9, 1 - p)))) of each genotype probability */
+int pb_test_vcf_qual(const float *h_p, int64_t n, int32_t *h_qual);
+
 #ifdef __cplusplus
 }
 #endif

@@ -7,10 +7,12 @@ inflate on the GPU: `pb_bam_fetch` -> batched `get_reads` (+ reservoir sampling)
 """
 from __future__ import annotations
 
+import ctypes as C
 import re
 
 import numpy as np
 
+from . import _lib
 from .bamio import BamReader, FastaReader
 from ._lib import PepperB200Error
 from .abi import PB_ERR_CAPACITY
@@ -225,11 +227,12 @@ class VariantFromFiles(_FromFiles):
 
     def call_stream(self, contig: str, intervals: list[tuple[int, int]], params: dict, batch: int = 32, capacity: int | None = None,
                     include_supplementary: bool = False, min_mapq: int = 0, downsample_rate: float = 1.0,
-                    max_reads: int = VARIANT_MAX_READS, want_images: bool = False) -> VariantCalls:
+                    max_reads: int = VARIANT_MAX_READS, want_images: bool = False, _finish=None) -> VariantCalls:
         """The whole interval list as ONE streaming session (pipeline.VariantStream): batch k+1's BGZF blocks are read, copied and
         inflated (helper thread, second reader, its own CUDA stream) while batch k's get_reads / encoder / network kernels run;
         candidates accumulate on the device and the network runs over whole 9,472-candidate chunks across batch boundaries.
-        `region_of` counts intervals from the start of the list."""
+        `region_of` counts intervals from the start of the list.  `_finish(session, n)`, when given, replaces the D2H fetch of the
+        candidates (they are still in the session's device buffers) and its result is returned."""
         from concurrent.futures import ThreadPoolExecutor
         if not intervals:
             raise ValueError("no intervals")
@@ -283,7 +286,7 @@ class VariantFromFiles(_FromFiles):
                         done += len(g)
                 t0 = time.perf_counter()
                 n = s.end()
-                out = s.fetch(n, want_images=want_images)
+                out = s.fetch(n, want_images=want_images) if _finish is None else _finish(s, n)
                 prof["end_fetch"] = time.perf_counter() - t0
                 self.last_profile = {k: round(v * 1e3, 2) for k, v in prof.items()}      # host wall time (ms) per stage of the last call
                 return out
@@ -291,6 +294,71 @@ class VariantFromFiles(_FromFiles):
                 if ex.rc != PB_ERR_CAPACITY:
                     raise
                 cap *= 2
+
+
+    def genome_table(self, contig: str, intervals: list[tuple[int, int]]) -> RegionTable:
+        """The region table + reference of a whole interval list, rows as the streaming session's groups build them."""
+        rows, spans = [], []
+        for (a, b) in intervals:
+            rs, re_ = max(0, a - REGION_SAFE_BASES), b + REGION_SAFE_BASES
+            rows.append([rs, re_, a, b, 0, 0, 0, 0]); spans.append((rs, re_ + 1))
+        return self._ref_table(contig, rows, spans)
+
+    def vcf_job(self, region: str | None = None, exclude=()) -> list[tuple[str, int, int]]:
+        return variant_job(self.fasta_contigs(), self.bam.get_chromosome_sequence_names(), region, exclude)
+
+    def fasta_contigs(self) -> list[tuple[str, int]]:
+        return [(c, self.fasta.get_chromosome_sequence_length(c)) for c in self.fasta.get_chromosome_names()]
+
+    def call_genome(self, out_dir: str, sample_name: str, region: str | None = None, exclude=(), params: dict | None = None,
+                    options: dict | None = None, vcf_options: dict | None = None, batch: int = 32, **kw) -> tuple:
+        """`pepper_variant call_variant -b -f -o -s [-r]` on this GPU: make_images + run_inference for every contig of the job
+        (variant_job), then per contig the candidate selection, site assembly and VCF text on the device over the session's
+        candidate buffers (pb_variant_vcf_device; only the text and its line table come back), then write_vcfs.  Writes the five
+        PEPPER_VARIANT_*.vcf.gz (+ .tbi) under `out_dir`; returns the totals of FindCandidates.py:185-189 (all, PEPPER, selected
+        for re-genotyping, of them SNPs, indels)."""
+        import time
+        import torch
+        from .abi import PbCandidateColumns, regions_array
+        from .candidates import ONT_OPTIONS
+        from .synth import ont_params
+        from .vcf import order_lines, vcf_text_device, write_vcfs
+        job = self.vcf_job(region, exclude)
+        names = [c for c, _, _ in job]
+        params = params or ont_params()
+        parts = []
+        prof = dict(calls=0.0, vcf=0.0, write=0.0, encoder_device=0.0, network_device=0.0)
+        dev = torch.device("cuda", self.device)
+        for cid, (contig, start, end) in enumerate(job):
+            intervals = variant_intervals(start, end)
+            if not intervals:
+                continue
+            table = self.genome_table(contig, intervals)
+
+            def finish(s, n, table=table, cid=cid):
+                dev_ms = self.caller.timings()                              # the session's encoder / network device time
+                prof["encoder_device"] += dev_ms["encode_ms"] / 1e3; prof["network_device"] += dev_ms["network_ms"] / 1e3
+                t0 = time.perf_counter()
+                cols, d_probs = PbCandidateColumns(), C.c_void_p()
+                _lib.check(s.L.pb_variant_stream_columns(self.caller.enc.h, C.byref(cols), C.byref(d_probs), None), "columns")
+                d_regions = torch.from_numpy(regions_array(table)[1]).to(dev)
+                d_ref = torch.from_numpy(np.ascontiguousarray(table.ref, np.uint8)).to(dev)
+                out = vcf_text_device(names, np.full(table.n_regions, cid, np.int32), cols, d_probs.value or 0, n, d_regions.data_ptr(),
+                                      d_ref.data_ptr(), options or ONT_OPTIONS, vcf_options, self.device)
+                prof["vcf"] += time.perf_counter() - t0
+                return out
+            t0 = time.perf_counter()
+            parts.append(self.call_stream(contig, intervals, params, batch, _finish=finish, **kw))
+            prof["calls"] += time.perf_counter() - t0
+        t0 = time.perf_counter()
+        text, lines = order_lines(parts, names)
+        totals = write_vcfs(out_dir, sample_name, self.fasta_contigs(), names, text, lines)
+        prof["write"] = time.perf_counter() - t0
+        prof["calls"] -= prof["vcf"]
+        # ms per stage of the last call: host wall of the sessions, of the VCF pass (synchronous) and of the writer; device time
+        # of the encoder and the network
+        self.last_genome_profile = {k: round(v * 1e3, 2) for k, v in prof.items()}
+        return totals
 
 
 class VariantFileSource(_FromFiles):
@@ -431,6 +499,51 @@ def polish_job(fasta_contigs: list[tuple[str, int]], bam_contigs: list[str], con
         regions.extend(polish_intervals(0, lengths[c] - 1))
     first.append(len(regions))
     return list(contigs), regions, first
+
+
+def parse_region(region: str) -> list[tuple[str, tuple[int, int] | None]]:
+    """`-r/--region` of call_variant (ImageGenerationUI.get_chromosome_list, pepper_variant ImageGenerationUI.py:131-171): a comma
+    list of `contig` or `contig:start-end`, where a name such as `chr1-3` expands to chr1, chr2, chr3."""
+    out = []
+    for name in [x.strip() for x in region.strip().split(",")]:
+        span = None
+        if ":" in name:
+            parts = name.strip().split(":")
+            if len(parts) != 2:
+                raise ValueError("--region: invalid value %r" % name)
+            name, rng = parts
+            span = [int(x) for x in rng.strip().split("-")]
+            if len(span) != 2 or not span[0] <= span[1]:
+                raise ValueError("--region: invalid value %r" % rng)
+            span = (span[0], span[1])
+        pieces = name.split("-")
+        if len(pieces) > 1:
+            prefix = re.match(r"\D*", name).group(0)
+            nums = sorted(int("".join(ch for ch in p if ch.isdigit())) for p in pieces)
+            out += [(prefix + str(k), span) for k in range(nums[0], nums[-1] + 1)]
+        else:
+            out.append((name, span))
+    return out
+
+
+def variant_job(fasta_contigs: list[tuple[str, int]], bam_contigs: list[str], region: str | None = None, exclude=()):
+    """The contigs a genome-wide call_variant processes, as (contig, start, end) intervals to tile with variant_intervals
+    (ImageGenerationUI.generate_images, pepper_variant ImageGenerationUI.py:283-316): without `region`, every contig common to the
+    FASTA and the BAM and not in `exclude`, in natural order, over [0, length - 1]; with it, the listed contigs in the listed order,
+    each span clamped to [0, length - 1]."""
+    lengths = dict(fasta_contigs)
+    if region is None:
+        common = sorted((set(lengths) & set(bam_contigs)) - set(exclude), key=natural_key)
+        if not common:
+            raise ValueError("no contig common to the BAM and the FASTA")
+        return [(c, 0, lengths[c] - 1) for c in common]
+    job = []
+    for c, span in parse_region(region):
+        if c not in lengths:
+            raise ValueError("--region: contig %r is not in the FASTA" % c)
+        s, e = span if span is not None else (0, lengths[c] - 1)
+        job.append((c, max(0, s), min(e, lengths[c] - 1)))
+    return job
 
 
 class PolishFileSource(_FromFiles):

@@ -13,10 +13,14 @@ count via reduceat) plus one pass that formats the records.  Output: one dict pe
 reference hands to pysam's `new_record` and `files`, the VCFs it is written to — a pysam writer consumes them unchanged."""
 from __future__ import annotations
 
+import ctypes as C
 import math
+import struct
 
 import numpy as np
 
+from . import _lib
+from .abi import PB_ERR_CAPACITY
 from .candidates import F_DV, F_REPEAT, F_SWAP, select_flags
 from .synth import RegionTable
 
@@ -152,3 +156,244 @@ def format_vcf_line(rec: dict, sample_fields=("GT", "AP", "GQ", "DP", "AD", "VAF
     sample = [("/".join(str(x) for x in rec["GT"]))] + [fmt(rec[f]) for f in sample_fields[1:]]
     return "\t".join([rec["contig"], str(rec["start"] + 1), ".", rec["alleles"][0], ",".join(rec["alleles"][1:]), str(rec["qual"]),
                       rec["filter"], ".", ":".join(sample_fields), ":".join(sample)])
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# Whole-genome VCF output: the GPU turns each contig's records into VCF text (pb_variant_vcf_*); the writer below orders the lines
+# as VCFWriter.write_vcf_records does, splits them into the reference's five files, and writes BGZF + a tabix index.
+
+class PbVcfOptions(C.Structure):
+    _fields_ = [("allowed_multiallelics", C.c_int32), ("reserved", C.c_int32), ("snp_q_cutoff", C.c_double),
+                ("indel_q_cutoff", C.c_double), ("snp_q_cutoff_in_lc", C.c_double), ("indel_q_cutoff_in_lc", C.c_double)]
+
+
+class PbVcfJob(C.Structure):
+    _fields_ = [("contig_of_region", C.c_void_p), ("names", C.c_void_p), ("name_off", C.c_void_p), ("vaf_table", C.c_void_p)]
+
+
+# pb_vcf_line_t; cls: 0 = pepper, 1 = variant-calling SNP, 2 = variant-calling indel
+VCF_LINE = np.dtype([("pos", np.int64), ("text_off", np.int64), ("contig", np.int32), ("ref_len", np.int32), ("cls", np.int32),
+                     ("text_len", np.int32)])
+CLASS_PEPPER, CLASS_VC_SNP, CLASS_VC_INDEL = 0, 1, 2
+VCF_FILES = ("PEPPER_VARIANT_FULL", "PEPPER_VARIANT_OUTPUT_PEPPER", "PEPPER_VARIANT_OUTPUT_VARIANT_CALLING",
+             "PEPPER_VARIANT_OUTPUT_VARIANT_CALLING_SNPs", "PEPPER_VARIANT_OUTPUT_VARIANT_CALLING_INDEL")
+_VAF_TABLE = None
+
+
+def vaf_table() -> np.ndarray:
+    """[256, 256, 8] NUL-padded text of round(ad / max(1, dp), 3) as format_vcf_line prints it, at [ad, dp] (AD and DP are the
+    encoder's uint8 counts).  Python's rounding of that quotient is kept on the host rather than restated on the device."""
+    global _VAF_TABLE
+    if _VAF_TABLE is None:
+        t = np.zeros((256, 256), dtype="S8")
+        for ad in range(256):
+            t[ad] = [("%.6g" % round(ad / max(1, dp), 3)).encode() for dp in range(256)]
+        _VAF_TABLE = np.ascontiguousarray(t).view(np.uint8).reshape(256, 256, 8)
+    return _VAF_TABLE
+
+
+def vcf_options(options: dict) -> PbVcfOptions:
+    return PbVcfOptions(int(options["allowed_multiallelics"]), 0, *(float(options[k]) for k in
+                        ("snp_q_cutoff", "indel_q_cutoff", "snp_q_cutoff_in_lc", "indel_q_cutoff_in_lc")))
+
+
+def _names_blob(names: list[str]):
+    enc = [n.encode() for n in names]
+    off = np.zeros(len(enc) + 1, np.int64)
+    off[1:] = np.cumsum([len(e) for e in enc])
+    return np.frombuffer(b"".join(enc) + b"\0", np.uint8).copy(), off
+
+
+def vcf_text_host(names: list[str], contig_of_region, positions, region_of, depths, freqs, keys_raw, probs, regions: RegionTable,
+                  options: dict, vcf_opts: dict | None = None, stream: int = 0):
+    """pb_variant_vcf_host: records on the host (any order; region r belongs to contig names[contig_of_region[r]]) -> (text uint8,
+    line table VCF_LINE) in (contig id, position) order."""
+    from .candidates import PbCandidateOptions
+    from .abi import regions_array, ALLELE_STRIDE
+    _lib.require_gpu()
+    L = _lib.lib()
+    vp = C.c_void_p
+    L.pb_variant_vcf_host.argtypes = [vp] * 6 + [C.c_int64, vp, C.c_int64, vp, C.c_int64, vp, vp, vp, C.c_int64, vp,
+                                                 C.POINTER(PbCandidateOptions), C.POINTER(PbVcfOptions), vp, C.c_int64, vp, C.c_int64,
+                                                 C.POINTER(C.c_int64), C.POINTER(C.c_int64), vp]
+    n = int(len(positions))
+    a = dict(pos=np.ascontiguousarray(positions, np.int64), rof=np.ascontiguousarray(region_of, np.int32),
+             dep=np.ascontiguousarray(depths, np.uint8), frq=np.ascontiguousarray(freqs, np.uint8),
+             keys=np.ascontiguousarray(keys_raw, np.uint8).reshape(n, ALLELE_STRIDE), pr=np.ascontiguousarray(probs, np.float32).reshape(n, 3))
+    regs, keep = regions_array(regions)
+    ref = np.ascontiguousarray(regions.ref, np.uint8)
+    cor = np.ascontiguousarray(contig_of_region, np.int32)
+    nm, off = _names_blob(names)
+    vt = vaf_table()
+    so, vo = PbCandidateOptions(**options), vcf_options(vcf_opts or VCF_OPTIONS_ONT)
+    text_cap, lines_cap = max(1, 160 * n), max(1, n)
+    while True:
+        text = np.empty(text_cap, np.uint8)
+        lines = np.empty(lines_cap, VCF_LINE)
+        nt, nl = C.c_int64(0), C.c_int64(0)
+        rc = L.pb_variant_vcf_host(a["pos"].ctypes.data, a["rof"].ctypes.data, a["dep"].ctypes.data, a["frq"].ctypes.data,
+                                   a["keys"].ctypes.data, a["pr"].ctypes.data, n, C.cast(regs, vp), regions.n_regions, ref.ctypes.data,
+                                   ref.shape[0], cor.ctypes.data, nm.ctypes.data, off.ctypes.data, len(names), vt.ctypes.data,
+                                   C.byref(so), C.byref(vo), text.ctypes.data, text_cap, lines.ctypes.data, lines_cap,
+                                   C.byref(nt), C.byref(nl), C.c_void_p(stream))
+        if rc == PB_ERR_CAPACITY:
+            text_cap, lines_cap = int(nt.value), int(nl.value)
+            continue
+        _lib.check(rc, "pb_variant_vcf_host")
+        return text[:nt.value], lines[:nl.value]
+
+
+def vcf_text_device(names: list[str], contig_of_region, cols, d_probs: int, n: int, d_regions: int, d_ref: int, options: dict,
+                    vcf_opts: dict | None = None, device: int = 0, stream: int = 0):
+    """pb_variant_vcf_device over records already in HBM (`cols`: abi.PbCandidateColumns of device pointers) -> (text uint8, line
+    table) on the host: only the VCF text and its line table leave the GPU."""
+    import torch
+    from .candidates import PbCandidateOptions
+    from .abi import PbCandidateColumns
+    L = _lib.lib()
+    vp = C.c_void_p
+    L.pb_variant_vcf_device.argtypes = [C.POINTER(PbCandidateColumns), vp, C.c_int64, vp, vp, C.POINTER(PbVcfJob),
+                                        C.POINTER(PbCandidateOptions), C.POINTER(PbVcfOptions), vp, C.c_int64, vp, C.c_int64,
+                                        C.POINTER(C.c_int64), C.POINTER(C.c_int64), vp]
+    dev = torch.device("cuda", device)
+    nm, off = _names_blob(names)
+    keep = [torch.from_numpy(x).to(dev) for x in (np.ascontiguousarray(contig_of_region, np.int32), nm, off, vaf_table().reshape(-1))]
+    job = PbVcfJob(*(t.data_ptr() for t in keep))
+    so, vo = PbCandidateOptions(**options), vcf_options(vcf_opts or VCF_OPTIONS_ONT)
+    text_cap, lines_cap = max(1, 160 * n), max(1, n)
+    while True:
+        text = torch.empty(text_cap, dtype=torch.uint8, device=dev)
+        lines = torch.empty(lines_cap * VCF_LINE.itemsize, dtype=torch.uint8, device=dev)
+        nt, nl = C.c_int64(0), C.c_int64(0)
+        rc = L.pb_variant_vcf_device(C.byref(cols), vp(d_probs), n, vp(d_regions), vp(d_ref), C.byref(job), C.byref(so), C.byref(vo),
+                                     vp(text.data_ptr()), text_cap, vp(lines.data_ptr()), lines_cap, C.byref(nt), C.byref(nl),
+                                     vp(stream))
+        if rc == PB_ERR_CAPACITY:
+            text_cap, lines_cap = int(nt.value), int(nl.value)
+            continue
+        _lib.check(rc, "pb_variant_vcf_device")
+        return (text[:nt.value].cpu().numpy(), lines[:nl.value * VCF_LINE.itemsize].cpu().numpy().view(VCF_LINE))
+
+
+def host_tail_text(records: list[dict], contig_id: int):
+    """The host tail's records of one contig (assemble_sites) -> (text, line table) through format_vcf_line: the same form as the
+    GPU's, so both go through one writer."""
+    txt = [(format_vcf_line(r) + "\n").encode() for r in records]
+    lines = np.zeros(len(records), VCF_LINE)
+    lines["pos"] = [r["start"] for r in records]
+    lines["contig"] = contig_id
+    lines["ref_len"] = [len(r["alleles"][0]) for r in records]
+    lines["cls"] = [CLASS_PEPPER if "pepper" in r["files"] else CLASS_VC_SNP if "variant_calling_snp" in r["files"] else CLASS_VC_INDEL
+                    for r in records]
+    lines["text_len"] = [len(t) for t in txt]
+    lines["text_off"] = np.concatenate([[0], np.cumsum(lines["text_len"])[:-1]]) if len(txt) else []
+    return np.frombuffer(b"".join(txt), np.uint8), lines
+
+
+def vcf_header(sample_name: str, fasta_contigs: list[tuple[str, int]]) -> str:
+    """The header VCFWriter.get_vcf_header declares (VcfWriter.py:220-289), each ID once, every FASTA contig in FAI order."""
+    h = ["##fileformat=VCFv4.2"]
+    for i, d in (("PASS", "All filters passed"), ("refCall", "Call is homozygous"), ("lowGQ", "Low genotype quality"),
+                 ("lowQUAL", "Low variant call quality"), ("conflictPos", "Overlapping record")):
+        h.append('##FILTER=<ID=%s,Description="%s">' % (i, d))
+    for i, n, t, d in (("GT", "1", "String", "Genotype"), ("DP", "1", "Integer", "Depth"), ("AD", "A", "Integer", "Allele depth"),
+                       ("VAF", "A", "Float", "Variant allele fractions."),
+                       ("AP", "A", "Float", "Maximum variant allele probability for each allele."),
+                       ("GQ", "1", "Float", "Genotype Quality"),
+                       ("REP", "1", "String", "If set to 1 then variant site is considered to be ina LowCompexity repeat region")):
+        h.append('##FORMAT=<ID=%s,Number=%s,Type=%s,Description="%s">' % (i, n, t, d))
+    h += ["##contig=<ID=%s,length=%d>" % (c, n) for c, n in fasta_contigs]
+    h.append("\t".join(["#CHROM", "POS", "ID", "REF", "ALT", "QUAL", "FILTER", "INFO", "FORMAT", sample_name]))
+    return "\n".join(h) + "\n"
+
+
+def order_lines(parts: list, names: list[str]):
+    """(text, lines) parts -> one text + line table in the order of write_vcf_records: sorted by (contig NAME, position)
+    (VcfWriter.py:144; lexical, so chr10 < chr2), and a site dropped when its position equals the previous written site's — the
+    reference never resets `last_position` between contigs (VcfWriter.py:151-152)."""
+    texts, tabs, base = [], [], 0
+    for text, lines in parts:
+        t = lines.copy()
+        t["text_off"] += base
+        base += text.shape[0]
+        texts.append(text); tabs.append(t)
+    text = np.concatenate(texts) if texts else np.zeros(0, np.uint8)
+    lines = np.concatenate(tabs) if tabs else np.zeros(0, VCF_LINE)
+    lex = np.empty(len(names), np.int64)
+    lex[np.array(sorted(range(len(names)), key=lambda i: names[i]), dtype=np.int64)] = np.arange(len(names))
+    lines = lines[np.lexsort((lines["pos"], lex[lines["contig"]]))]
+    keep = np.ones(lines.shape[0], bool)
+    keep[1:] = lines["pos"][1:] != lines["pos"][:-1]
+    return text, lines[keep]
+
+
+def _gather(text: np.ndarray, lines: np.ndarray) -> bytes:
+    """The bytes of `lines`, in table order: one slice per run of lines that lie back to back in the text (the whole of a contig's
+    part for the full file), so no per-byte index is built."""
+    if lines.shape[0] == 0:
+        return b""
+    off, ln = lines["text_off"], lines["text_len"].astype(np.int64)
+    brk = np.flatnonzero(off[1:] != off[:-1] + ln[:-1]) + 1
+    first, last = np.concatenate([[0], brk]), np.concatenate([brk, [lines.shape[0]]]) - 1
+    mv = memoryview(np.ascontiguousarray(text))
+    return b"".join(mv[a:b] for a, b in zip(off[first].tolist(), (off[last] + ln[last]).tolist()))
+
+
+BGZF_PAYLOAD = 0xff00
+
+
+def _bgzf(data: bytes, pool, level: int = 6):
+    """BGZF members of <= 65,280 bytes each (+ the EOF block) and the uncompressed start / compressed offset of each member."""
+    from .synth_files import _bgzf_block, BGZF_EOF
+    starts = list(range(0, len(data), BGZF_PAYLOAD))
+    blocks = list(pool.map(lambda s: _bgzf_block(data[s:s + BGZF_PAYLOAD], level), starts))
+    coff = np.concatenate([[0], np.cumsum([len(b) for b in blocks])]).astype(np.int64)
+    return b"".join(blocks) + BGZF_EOF, np.array(starts, np.int64), coff
+
+
+def _tabix(names: list[str], tids: np.ndarray, beg: np.ndarray, end: np.ndarray, ustart: np.ndarray, uend: np.ndarray,
+           blk_u: np.ndarray, blk_c: np.ndarray, eof_c: int, total_u: int) -> bytes:
+    """TBI of a VCF (format 2, col_seq 1, col_beg 2, col_end 0, meta '#'): the per-reference bins / chunks / 16 kb linear index
+    are those of a BAI (synth_files._bai_bytes) over [pos, pos + len(REF)) and the lines' virtual offsets."""
+    from .synth_files import _bai_bytes
+
+    u = np.concatenate([ustart, uend]).astype(np.int64)
+    k = np.maximum(np.searchsorted(blk_u, u, side="right") - 1, 0)
+    v = np.where(u >= total_u, np.int64(eof_c) << 16, (blk_c[k] << 16) | (u - blk_u[k]))
+    voff = dict(zip(u.tolist(), v.tolist())).__getitem__          # every line's virtual offsets from one searchsorted
+    spans = {}
+    for t, b, e, us, ue in zip(tids.tolist(), beg.tolist(), end.tolist(), ustart.tolist(), uend.tolist()):
+        spans.setdefault(t, []).append((b, e, us, ue))
+    nm = b"".join(n.encode() + b"\0" for n in names)
+    head = b"TBI\x01" + struct.pack("<8i", len(names), 2, 1, 2, 0, ord("#"), 0, len(nm)) + nm
+    return head + _bai_bytes(len(names), spans, voff)[8:]
+
+
+def write_vcfs(out_dir: str, sample_name: str, fasta_contigs: list[tuple[str, int]], names: list[str], text: np.ndarray,
+               lines: np.ndarray, threads: int = 8) -> tuple[int, int, int, int, int]:
+    """Ordered lines (order_lines) -> the five bgzipped, tabix-indexed VCFs of write_vcf_records under `out_dir`; returns its
+    totals (full, pepper, variant calling, variant-calling SNPs, indels)."""
+    import os
+    from concurrent.futures import ThreadPoolExecutor
+    os.makedirs(out_dir, exist_ok=True)
+    head = vcf_header(sample_name, fasta_contigs).encode()
+    cls = lines["cls"]
+    masks = (np.ones(cls.shape[0], bool), cls == CLASS_PEPPER, cls != CLASS_PEPPER, cls == CLASS_VC_SNP, cls == CLASS_VC_INDEL)
+    with ThreadPoolExecutor(max_workers=max(1, threads)) as pool:
+        for name, mask in zip(VCF_FILES, masks):
+            sel = lines[mask]
+            body = _gather(text, sel)
+            data = head + body
+            gz, blk_u, blk_c = _bgzf(data, pool)
+            path = os.path.join(out_dir, name + ".vcf.gz")
+            with open(path, "wb") as f:
+                f.write(gz)
+            # tabix reference ids: contigs in the order their lines appear
+            seen = list(dict.fromkeys(sel["contig"].tolist()))
+            tid_of = {c: i for i, c in enumerate(seen)}
+            us = len(head) + np.concatenate([[0], np.cumsum(sel["text_len"].astype(np.int64))])
+            tbi = _tabix([names[c] for c in seen], np.array([tid_of[c] for c in sel["contig"].tolist()], np.int64), sel["pos"],
+                         sel["pos"] + sel["ref_len"], us[:-1], us[1:], blk_u, blk_c, int(blk_c[-1]), len(data))
+            with open(path + ".tbi", "wb") as f:
+                f.write(_bgzf(tbi, pool)[0])
+    return tuple(int(m.sum()) for m in masks)

@@ -21,5 +21,6 @@ for tool in memcheck racecheck; do
     run inflate $tool tests/test_inflate_gpu.py tests/test_inflate_edges_gpu.py -k "inflate_matches or rejects or case_table or cut_short"   # k_bgzf_inflate
     run realign $tool tests/test_realign_edges_gpu.py -k "reject or (match_port and 8)"                # k_sw16<8>, k_banded
     run stitch_sink $tool tests/test_polish_assembly_gpu.py -k "stitch_sink"                           # k_stitch_sink
+    run vcf $tool tests/test_genome_vcf_gpu.py -k "vcf_host"                                         # k_site_sizes, k_site_write
 done
 cat "$OUT/sanitizer_summary.txt"
