@@ -122,6 +122,24 @@ static Dir empty_dir() {
 // ------------------------------------------------------------------------------------------------- variant
 constexpr int VT = 33, VH = 256;
 
+#ifdef PB_LSTM_TRACE
+// Timing build only: the stamps of the latest launch of each variant LSTM layer (layer 0 words, then layer 1), on the
+// device that ran it.  pb_lstm_trace_copy is exported by these builds alone (scripts/trace_lstm_layer.py).
+static uint64_t *g_lstm_trace = nullptr;
+static int lstm_trace_buffer(int layer, uint64_t **out) {
+    if (!g_lstm_trace) PB_CUDA(cudaMalloc(&g_lstm_trace, sizeof(uint64_t) * 2 * tc::lstm_trace_words(VT)));
+    *out = g_lstm_trace + layer * tc::lstm_trace_words(VT);
+    return PB_OK;
+}
+extern "C" int pb_lstm_trace_copy(uint64_t *host, int64_t n_words) {
+    if (!g_lstm_trace) { set_error("no k_lstm_layer launch has been traced"); return PB_ERR_STATE; }
+    if (n_words != 2 * tc::lstm_trace_words(VT)) { set_error("trace holds 2 x %lld words", (long long) tc::lstm_trace_words(VT)); return PB_ERR_ARG; }
+    PB_CUDA(cudaDeviceSynchronize());
+    PB_CUDA(cudaMemcpy(host, g_lstm_trace, sizeof(uint64_t) * n_words, cudaMemcpyDeviceToHost));
+    return PB_OK;
+}
+#endif
+
 // One bidirectional LSTM layer of the variant network over its 33 steps, reading T.img_op (layer 0) or T.yenc (layer 1)
 // and writing T.yenc / T.ydec (+ the optional fp32 copy y_f32 [B][33][512]); the cell state ends in T.c.  lo_x / lo_h:
 // the a_lo x w_hi product of the x-part / h-part runs (the int8 images of layer 0 have no lo operand).  persist: one
@@ -156,6 +174,10 @@ static int variant_lstm_layer_tc(pb_variant_net *N, int layer, int64_t B, bool l
         if (y_f32) { L.y_f32 = y_f32; L.ldy = (int64_t) VT * 512; }
         L.M = (int) B; L.n_mt = (int) Mt; L.T = VT; L.c_ld = Bp;
         L.lo_x = lo_x; L.lo_h = lo_h;
+#ifdef PB_LSTM_TRACE
+        PB_TRY(lstm_trace_buffer(layer, &L.trace));
+        PB_CUDA(cudaMemsetAsync(L.trace, 0, sizeof(uint64_t) * tc::lstm_trace_words(VT), st));
+#endif
         static bool attr_set = false;
         if (!attr_set) {
             PB_CUDA(cudaFuncSetAttribute(tc::k_lstm_layer, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::LSTM_SMEM_BYTES));

@@ -252,11 +252,10 @@ __device__ __forceinline__ void gates4(const float (&acc)[128], int i, float2 bz
     gt[2] = odd ? b0 : r0; gt[3] = odd ? b1 : r1;
 }
 // h of units (2i, 2i + 1) meet in lanes q and q ^ 2: the even-unit lane stores both (4 B operand words, 8 B fp32 pair)
-template <bool UNIT = false>
 __device__ __forceinline__ void store_h(float hn, bool store, op_t *y_hi, op_t *y_lo, int64_t o, float *y_f32) {
     uint32_t hi, lo;
     const float hn1 = __shfl_xor_sync(0xffffffffu, hn, 2);
-    split2<UNIT>(hn, hn1, hi, lo);
+    split2(hn, hn1, hi, lo);
     // predicated stores, no branch: a branch per cell would keep the scheduler from overlapping consecutive cells
     if (store) *reinterpret_cast<uint32_t *>(y_hi + o) = hi;
     if (store) *reinterpret_cast<uint32_t *>(y_lo + o) = lo;
@@ -388,7 +387,38 @@ struct LstmLayer {
     int M, n_mt, T;
     int64_t c_ld;
     int lo_x, lo_h;                    // 1: the a_lo x w_hi product of the x-part / h-part is executed (0: two products)
+#ifdef PB_LSTM_TRACE
+    uint64_t *trace;                   // lstm_trace_words(T) stamps per launch, nullptr: none
+#endif
 };
+
+#ifdef PB_LSTM_TRACE
+// Timing build only (-DPB_LSTM_TRACE; scripts/trace_lstm_layer.py): %clock64 stamps of CTAs 0, gridDim / 2 and
+// gridDim - 1.  Per sampled CTA, in 64-bit words (cw = consumer warp 0-7, nt = gate tile):
+//   [((cw * T + t) * 4 + nt) * 4 + k]  k: 0 tile start, 1 first bar_full passed, 2 wg_wait<0> returned, 3 epilogue end
+//   [128 T + (cw * T + t) * 2 + k]     k: 0 __threadfence returned, 1 bar_h arrived
+//   [144 T + t * 3 + k]                producer, t >= 1; k: 0 bar_h wait start, 1 wait end, 2 first h-part copy issued
+//   [147 T + k]                        k: 0 %globaltimer, 1 %clock64 at the start; 2, 3 the same when warp 0 ends
+constexpr int LSTM_TRACE_CTAS = 3;
+__host__ __device__ constexpr int64_t lstm_trace_cta_words(int T) { return 147 * (int64_t) T + 4; }
+__host__ __device__ constexpr int64_t lstm_trace_words(int T) { return LSTM_TRACE_CTAS * lstm_trace_cta_words(T); }
+__device__ __forceinline__ uint64_t trace_clock() {
+    uint64_t c;
+    asm volatile("mov.u64 %0, %%clock64;" : "=l"(c) :: "memory");
+    return c;
+}
+__device__ __forceinline__ uint64_t trace_gtime() {
+    uint64_t c;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(c) :: "memory");
+    return c;
+}
+#define LSTM_STAMP(off)                                          \
+    do {                                                         \
+        if (tr && lane == 0) tr[off] = trace_clock();            \
+    } while (0)
+#else
+#define LSTM_STAMP(off) do {} while (0)
+#endif
 
 __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
     extern __shared__ __align__(128) uint8_t smem[];
@@ -406,6 +436,11 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     for (int i = threadIdx.x; i < 4 * PBN; i += LSTM_THREADS) sbias[i] = G.bias[dir][i];
+#ifdef PB_LSTM_TRACE
+    const int ts = blockIdx.x == 0 ? 0 : blockIdx.x == gridDim.x / 2 ? 1 : blockIdx.x == gridDim.x - 1 ? 2 : -1;
+    uint64_t *const tr = G.trace && ts >= 0 ? G.trace + ts * lstm_trace_cta_words(G.T) : nullptr;
+    if (tr && threadIdx.x == 0) { tr[147 * G.T] = trace_gtime(); tr[147 * G.T + 1] = trace_clock(); }
+#endif
     __syncthreads();
 
     if (warp >= CONS_WARPS) {
@@ -425,14 +460,17 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
                             const int kk = kt - G.x_nkt;
                             if (kk == 0 && nt == 0) {
                                 // every consumer warp has written its part of h_{t-1}: make it visible to the bulk-copy engine
+                                LSTM_STAMP(144 * G.T + t * 3);
                                 mbar_wait(bar_h, (uint32_t) (t - 1) & 1u);
                                 asm volatile("fence.proxy.async;" ::: "memory");
+                                LSTM_STAMP(144 * G.T + t * 3 + 1);
                             }
                             const int64_t off = (int64_t) mt * G.y_mt_stride + ((int64_t) tp * 16 + dir * 8 + kk) * TILE_ELEMS;
                             a_hi = G.y_hi + off; a_lo = G.lo_h ? G.y_lo + off : nullptr;
                         }
                         const int64_t woff = ((int64_t) nt * w_nkt + kt) * WTILE_ELEMS;
                         load_stage(smem_base, bar_full, bar_empty, g, a_hi, a_lo, G.w_hi[dir] + woff, G.w_lo[dir] + woff);
+                        if (t > 0 && nt == 0 && kt == G.x_nkt) LSTM_STAMP(144 * G.T + t * 3 + 2);
                     }
                 }
             }
@@ -454,37 +492,67 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
         const int nkt = G.x_nkt + (t > 0 ? 8 : 0);
         const int64_t y0 = (int64_t) mt * G.y_mt_stride + (int64_t) (tt * 16 + dir * 8) * TILE_ELEMS + r128 * 8;
         for (int nt = 0; nt < 4; nt++) {
+#ifdef PB_LSTM_TRACE
+            const int tc0 = ((warp * G.T + t) * 4 + nt) * 4;
+#endif
+            LSTM_STAMP(tc0);
             // cell states of units nt * 64 + 2 i + q / 2, in flight during the k-loop
             float *cp = G.c[dir] + (int64_t) (nt * (PBN / 4) + (q >> 1)) * G.c_ld + row;
             float c_prev[PBN / 8];
 #pragma unroll
             for (int i = 0; i < PBN / 8; i++) c_prev[i] = valid ? __ldcg(cp + i * c2) : 0.f;
+#ifdef PB_LSTM_TRACE
+            mbar_wait(bar_full + 8 * (g % PSTAGES), (g / PSTAGES) & 1u);     // mma_tile's first wait then passes at once
+            LSTM_STAMP(tc0 + 1);
+#endif
             mma_tile(acc, smem_base, bar_full, bar_empty, g, nkt, G.x_nkt, lo_x, lo_h, wg, lane);
+            LSTM_STAMP(tc0 + 2);
             // the stores recompute their addresses (IMAD per cell) instead of keeping the 32 load pointers alive across
             // the k-loop
             int c2s;
             asm volatile("mov.b32 %0, %1;" : "=r"(c2s) : "r"(c2));
             const float *sb = sbias + nt * PBN + 2 * q;
-            // units nt * 64 .. + 63 are operand k-tiles 2 nt, 2 nt + 1 of this step
-            op_t *yh = G.y_hi + y0 + 2 * nt * TILE_ELEMS, *yl = G.y_lo + y0 + 2 * nt * TILE_ELEMS;
-            float *yf = G.y_f32 ? G.y_f32 + (int64_t) row * G.ldy + (int64_t) tt * 512 + dir * 256 + nt * (PBN / 4) + (q >> 1) : nullptr;
+            // units nt * 64 .. + 63 are operand k-tiles 2 nt, 2 nt + 1 of this step.  Lanes q and q ^ 2 hold units 2 i and
+            // 2 i + 1 of the same row: the even-unit lane writes the hi words of the pair, the odd-unit lane the lo words.
+            const bool odd_u = q >> 1;
+            op_t *yw = (odd_u ? G.y_lo : G.y_hi) + y0 + 2 * nt * TILE_ELEMS;
+            float *yf = G.y_f32 ? G.y_f32 + (int64_t) row * G.ldy + (int64_t) tt * 512 + dir * 256 + nt * (PBN / 4) : nullptr;
 #pragma unroll
-            for (int i = 0; i < PBN / 8; i++) {
-                float gt[4];
-                gates4(acc, i, *reinterpret_cast<const float2 *>(sb + 8 * i), inv_s, q, gt);
-                const float cn = sigm(gt[1]) * c_prev[i] + sigm(gt[0]) * tanh_fast(gt[2]);
-                const float hn = sigm(gt[3]) * tanh_fast(cn);
-                if (valid) cp[i * c2s] = cn;
-                // element (unit nt * 64 + 2 i, row r128) of the step's operand tiles, relative to the lane's base
-                store_h<true>(hn, valid && !(q & 2), yh, yl, (i >> 4) * TILE_ELEMS + ((i & 15) >> 2) * 1024 + 2 * (i & 3),
-                              yf ? yf + 2 * i : nullptr);
+            for (int m = 0; m < PBN / 16; m++) {
+                // cells i = 2 m, 2 m + 1: their two 4 B operand words are adjacent in row r128 and go out as one 8 B store
+                // (lanes 4 apart fill the other half of the 32 B sector); four cells per 16 B store need registers the
+                // 168-register launch does not have (68 B of spills)
+                uint32_t w[2];
+#pragma unroll
+                for (int e = 0; e < 2; e++) {
+                    const int i = 2 * m + e;
+                    float gt[4];
+                    gates4(acc, i, *reinterpret_cast<const float2 *>(sb + 8 * i), inv_s, q, gt);
+                    const float cn = sigm(gt[1]) * c_prev[i] + sigm(gt[0]) * tanh_fast(gt[2]);
+                    const float hn = sigm(gt[3]) * tanh_fast(cn);
+                    if (valid) cp[i * c2s] = cn;
+                    const float hp = __shfl_xor_sync(0xffffffffu, hn, 2);
+                    const float h0 = odd_u ? hp : hn, h1 = odd_u ? hn : hp;          // units 2 i, 2 i + 1
+                    uint32_t hi, lo;
+                    split2<true>(h0, h1, hi, lo);
+                    w[e] = odd_u ? lo : hi;
+                    if (yf && valid && !odd_u) *reinterpret_cast<float2 *>(yf + 2 * i) = make_float2(h0, h1);
+                }
+                // element (unit nt * 64 + 4 m, row r128) of the step's operand tiles, relative to the lane's base
+                if (valid) __stwb(reinterpret_cast<uint2 *>(yw + (m >> 3) * TILE_ELEMS + ((m >> 1) & 3) * 1024 + 4 * (m & 1)), make_uint2(w[0], w[1]));
             }
+            LSTM_STAMP(tc0 + 3);
         }
         // h_t of this warp's rows is complete (all four gate tiles): publish it to the producer thread
         __threadfence();
+        LSTM_STAMP(128 * G.T + (warp * G.T + t) * 2);
         __syncwarp();
         if (lane == 0) mbar_arrive(bar_h);
+        LSTM_STAMP(128 * G.T + (warp * G.T + t) * 2 + 1);
     }
+#ifdef PB_LSTM_TRACE
+    if (tr && threadIdx.x == 0) { tr[147 * G.T + 2] = trace_gtime(); tr[147 * G.T + 3] = trace_clock(); }
+#endif
 }
 
 // ---------------------------------------------------------------- persistent GRU layer kernel (polish)
