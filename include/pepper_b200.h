@@ -646,12 +646,15 @@ typedef struct {
     int32_t text_len;     /* bytes of the line, '\n' included */
 } pb_vcf_line_t;
 /* device arrays: contig id per region id, contig names back to back with name_off [n_contigs + 1],
- * vaf_table [256][256][8]: NUL-padded "%g" of round(ad / max(1, dp), 3) at [ad][dp] */
+ * vaf_table [256][256][8]: NUL-padded "%g" of round(ad / max(1, dp), 3) at [ad][dp],
+ * window (optional) [n_regions][2]: the positions [lo, hi] a region's records may form sites at; a record outside its
+ * region's window takes part in no site.  NULL keeps every record. */
 typedef struct {
     const int32_t *contig_of_region;
     const char    *names;
     const int64_t *name_off;
     const char    *vaf_table;
+    const int64_t *window;
 } pb_vcf_job_t;
 /* Every record of the columns (device) -> text (device, text_cap bytes) + line table (device, lines_cap).
  * *n_text / *n_lines: the exact need.  PB_ERR_CAPACITY when d_text / d_lines is NULL or short (nothing written). */
@@ -672,6 +675,23 @@ int pb_variant_vcf_host(const int64_t *h_positions, const int32_t *h_region_of, 
 int pb_test_format_g(const float *h_x, int64_t n, char *h_out);
 /* diagnostics: h_qual [n], the device's QUAL = max(1, int(-10 log10(max(1e-9, 1 - p)))) of each genotype probability */
 int pb_test_vcf_qual(const float *h_p, int64_t n, int32_t *h_qual);
+/* Lays lines out back to back: line sel[i] of d_lines (its text_len bytes at text_off in d_text) goes to d_out + dst[i].
+ * d_sel / d_dst [n] are device arrays. */
+int pb_vcf_gather_lines_device(const char *d_text, const pb_vcf_line_t *d_lines, const int64_t *d_sel, const int64_t *d_dst,
+                               int64_t n, uint8_t *d_out, void *stream);
+
+/* ------------------------------------------------------------------------
+ * BGZF compression on the GPU (SAMv1 §4.1).  Member k is the payload bytes [member_off[k], member_off[k+1]) (at most
+ * 65,280) and becomes one complete BGZF member: gzip header with BSIZE, raw DEFLATE (one dynamic Huffman block with a
+ * 32 KiB window inside the member, or one stored block when that is not smaller), CRC32, ISIZE.  The members are written
+ * back to back to d_out; h_member_bytes [n_members] receives each member's size and *n_out the total.  PB_ERR_CAPACITY
+ * (with *n_out = the bytes needed) when d_out is NULL or out_cap is short.  h_member_off [n_members + 1] is a host array.
+ * ---------------------------------------------------------------------- */
+int pb_bgzf_compress_device(const uint8_t *d_payload, const int64_t *h_member_off, int64_t n_members, uint8_t *d_out,
+                            int64_t out_cap, int64_t *h_member_bytes, int64_t *n_out, void *stream);
+/* the same over host buffers (h_member_off indexes h_payload) */
+int pb_bgzf_compress_host(const uint8_t *h_payload, const int64_t *h_member_off, int64_t n_members, uint8_t *h_out,
+                          int64_t out_cap, int64_t *h_member_bytes, int64_t *n_out, void *stream);
 
 #ifdef __cplusplus
 }

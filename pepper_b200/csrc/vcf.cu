@@ -291,11 +291,25 @@ __device__ int64_t site_line(const VcfArgs &A, int64_t s, char *out, pb_vcf_line
 }
 
 __global__ void k_site_keys(const int64_t *__restrict__ pos, const int32_t *__restrict__ rof, const int32_t *__restrict__ contig_of_region,
-                            const uint8_t *__restrict__ flags, int64_t n, int64_t *__restrict__ key, int64_t *__restrict__ iota) {
+                            const int64_t *__restrict__ window, uint8_t *__restrict__ flags, int64_t n, int64_t *__restrict__ key,
+                            int64_t *__restrict__ iota) {
     const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    // a record outside its region's window counts as not selected, so the INT64_MAX site it joins still writes no line
+    if (window && (pos[i] < window[2 * rof[i]] || pos[i] > window[2 * rof[i] + 1])) flags[i] &= (uint8_t) ~F_DV;
     key[i] = (flags[i] & F_DV) ? (((int64_t) contig_of_region[rof[i]] << 40) | pos[i]) : INT64_MAX;
     iota[i] = i;
+}
+
+__global__ void k_gather_lines(const char *__restrict__ text, const pb_vcf_line_t *__restrict__ lines, const int64_t *__restrict__ sel,
+                               const int64_t *__restrict__ dst, int64_t n, uint8_t *__restrict__ out) {
+    const int64_t w = ((int64_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5;     // one warp per line
+    const int lane = threadIdx.x & 31;
+    if (w >= n) return;
+    const pb_vcf_line_t ln = lines[sel[w]];
+    const char *s = text + ln.text_off;
+    uint8_t *d = out + dst[w];
+    for (int k = lane; k < ln.text_len; k += 32) d[k] = (uint8_t) s[k];
 }
 
 __global__ void k_site_heads(const int64_t *__restrict__ key, int64_t n, int32_t *__restrict__ head) {
@@ -362,8 +376,8 @@ extern "C" int pb_variant_vcf_device(const pb_candidate_columns_t *cols, const f
                                                  d_regions, d_ref, sel_opt, flags.as<uint8_t>(), geno.as<uint8_t>(), stream_));
         PB_TRY(key.reserve(8 * n)); PB_TRY(key2.reserve(8 * n)); PB_TRY(idx.reserve(8 * n)); PB_TRY(order.reserve(8 * n));
         const unsigned gb = (unsigned) ceil_div(n, 256);
-        k_site_keys<<<gb, 256, 0, st>>>(cols->positions, cols->region_of, job->contig_of_region, flags.as<uint8_t>(), n, key.as<int64_t>(),
-                                        idx.as<int64_t>());
+        k_site_keys<<<gb, 256, 0, st>>>(cols->positions, cols->region_of, job->contig_of_region, job->window, flags.as<uint8_t>(), n,
+                                        key.as<int64_t>(), idx.as<int64_t>());
         size_t tb = 0;
         PB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, key.as<int64_t>(), key2.as<int64_t>(), idx.as<int64_t>(), order.as<int64_t>(),
                                                 (int) n, 0, 64, st));
@@ -438,7 +452,7 @@ extern "C" int pb_variant_vcf_host(const int64_t *h_positions, const int32_t *h_
         PB_TRY(upload(vt, h_vaf_table, 256 * 256 * VAF_STRIDE, st));
         PB_TRY(tx.reserve(text_cap > 0 ? text_cap : 1)); PB_TRY(ln.reserve(sizeof(pb_vcf_line_t) * (lines_cap > 0 ? lines_cap : 1)));
         pb_candidate_columns_t cols{p.as<int64_t>(), r.as<int32_t>(), d.as<uint8_t>(), f.as<uint8_t>(), k.as<char>()};
-        pb_vcf_job_t job{cr.as<int32_t>(), nm.as<char>(), no.as<int64_t>(), vt.as<char>()};
+        pb_vcf_job_t job{cr.as<int32_t>(), nm.as<char>(), no.as<int64_t>(), vt.as<char>(), nullptr};
         PB_TRY(pb_variant_vcf_device(&cols, pr.as<float>(), n, rg.as<pb_region_t>(), rf.as<char>(), &job, sel_opt, vcf_opt,
                                      h_text ? tx.as<char>() : nullptr, text_cap, h_lines ? ln.as<pb_vcf_line_t>() : nullptr, lines_cap,
                                      n_text, n_lines, stream_));
@@ -451,6 +465,15 @@ extern "C" int pb_variant_vcf_host(const int64_t *h_positions, const int32_t *h_
     DevBuf *bufs[] = {&p, &r, &d, &f, &k, &pr, &rg, &rf, &cr, &nm, &no, &vt, &tx, &ln};
     for (auto *b : bufs) b->release();
     return rc;
+}
+
+extern "C" int pb_vcf_gather_lines_device(const char *d_text, const pb_vcf_line_t *d_lines, const int64_t *d_sel, const int64_t *d_dst,
+                                          int64_t n, uint8_t *d_out, void *stream_) {
+    if (n <= 0) return PB_OK;
+    if (!d_text || !d_lines || !d_sel || !d_dst || !d_out) { set_error("null argument"); return PB_ERR_ARG; }
+    k_gather_lines<<<(unsigned) ceil_div(n * 32, 256), 256, 0, (cudaStream_t) stream_>>>(d_text, d_lines, d_sel, d_dst, n, d_out);
+    PB_CUDA(cudaGetLastError());
+    return PB_OK;
 }
 
 extern "C" int pb_test_format_g(const float *h_x, int64_t n, char *h_out) {

@@ -15,6 +15,8 @@ Two schedules:
 Backend-agnostic (`nccl` on GPUs, `gloo` in the CPU tests)."""
 from __future__ import annotations
 
+import ctypes as C
+
 import numpy as np
 
 from .abi import PRED_RECORD
@@ -528,3 +530,408 @@ def assemble_contigs(data: np.ndarray, segments: list[tuple[int, int]], group_co
         parts[group_contig[g]].append(bytes(data[off:off + k]))
         off += k
     return {c: b"".join(p).decode() for c, p in parts.items()}
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# Whole-genome variant calling across ranks: BAM + FASTA in, the five indexed VCFs of `pepper_variant call_variant` out.
+
+# the group table every rank publishes: per group [ran, lines, first position, last position, PEPPER lines, variant-calling
+# SNP lines, indel lines, class of the first line]
+GT_RAN, GT_LINES, GT_FIRST, GT_LAST, GT_PEPPER, GT_SNP, GT_INDEL, GT_FIRST_CLS = range(8)
+NO_BOUNDARY = -1
+
+
+class ListClaimer:
+    """Hands out a fixed list of group ids: a rank's share given in advance (GroupClaimer's interface)."""
+
+    def __init__(self, ids):
+        self._it = iter([int(g) for g in ids])
+
+    def next(self):
+        return next(self._it, None)
+
+
+class GenomeRankPart:
+    """One rank's share of a genome call between the collectives: the groups it ran, the boundary records it held back
+    (PRED_RECORD), its VCF text (device) and line table (host, VCF_LINE), each line's group, and the edge lines of the boundaries
+    whose later group it owns."""
+
+    def __init__(self):
+        self.groups, self.held = [], np.zeros(0, PRED_RECORD)
+        self.text, self.lines, self.line_group = None, None, np.zeros(0, np.int64)
+        self.edges = {}
+        self.meta, self.comp = b"", None
+        self.phase_ms = {}
+
+
+def group_table_rows(part: GenomeRankPart, n_groups: int) -> np.ndarray:
+    """This rank's rows of the group table (zeros for the groups it did not run), edge lines counted as their later group's
+    first line."""
+    from .vcf import CLASS_PEPPER, CLASS_VC_SNP, CLASS_VC_INDEL
+    t = np.zeros((n_groups, 8), np.int64)
+    for g in part.groups:
+        pos, cls = group_lines(part, g)
+        t[g, GT_RAN] = 1
+        t[g, GT_LINES] = pos.shape[0]
+        if pos.shape[0]:
+            t[g, GT_FIRST], t[g, GT_LAST], t[g, GT_FIRST_CLS] = pos[0], pos[-1], cls[0]
+            t[g, GT_PEPPER] = int((cls == CLASS_PEPPER).sum())
+            t[g, GT_SNP] = int((cls == CLASS_VC_SNP).sum())
+            t[g, GT_INDEL] = int((cls == CLASS_VC_INDEL).sum())
+    return t
+
+
+def group_lines(part: GenomeRankPart, g: int):
+    """(positions, classes) of group g's lines in file order: its edge line, then the lines of its own VCF pass."""
+    own = part.lines[part.line_group == g] if part.lines is not None else np.zeros(0)
+    e = part.edges.get(g)
+    pos = np.concatenate([e[1]["pos"] if e else np.zeros(0, np.int64), own["pos"] if own.shape[0] else np.zeros(0, np.int64)])
+    cls = np.concatenate([e[1]["cls"] if e else np.zeros(0, np.int32), own["cls"] if own.shape[0] else np.zeros(0, np.int32)])
+    return pos.astype(np.int64), cls.astype(np.int32)
+
+
+def last_position_drops(table: np.ndarray, group_contig: np.ndarray, names: list[str]) -> np.ndarray:
+    """Groups whose first line write_vcf_records skips (VcfWriter.py:151-152: `last_position` is never reset, so a contig's first
+    line is dropped when its position equals that of the previous line in lexical contig order, whichever rank wrote it)."""
+    lex = np.empty(len(names), np.int64)
+    lex[np.array(sorted(range(len(names)), key=lambda i: names[i]), dtype=np.int64)] = np.arange(len(names))
+    drop = np.zeros(table.shape[0], bool)
+    prev = None
+    for g in sorted(range(table.shape[0]), key=lambda g: (lex[group_contig[g]], g)):
+        if table[g, GT_LINES] == 0:
+            continue
+        drop[g] = prev is not None and table[g, GT_FIRST] == prev
+        prev = table[g, GT_LAST]
+    return drop
+
+
+def genome_totals(table: np.ndarray, drop: np.ndarray) -> tuple[int, int, int, int, int]:
+    """The totals of FindCandidates.py:185-189 (all, PEPPER, variant calling, of them SNPs, indels) after the drops."""
+    from .vcf import CLASS_PEPPER, CLASS_VC_SNP, CLASS_VC_INDEL
+    fc = table[:, GT_FIRST_CLS]
+    d = drop.astype(np.int64)
+    pep = int(table[:, GT_PEPPER].sum() - (d * (fc == CLASS_PEPPER)).sum())
+    snp = int(table[:, GT_SNP].sum() - (d * (fc == CLASS_VC_SNP)).sum())
+    indel = int(table[:, GT_INDEL].sum() - (d * (fc == CLASS_VC_INDEL)).sum())
+    return int(table[:, GT_LINES].sum() - d.sum()), pep, snp + indel, snp, indel
+
+
+def parse_rank_bytes(data) -> dict:
+    """A rank's gathered bytes (GenomeRankPart.meta + .comp) -> {group id: vcf.GroupPart}."""
+    from .vcf import GROUP_LINE, GroupPart, member_cuts, file_masks
+    buf = memoryview(np.ascontiguousarray(data, np.uint8))
+    if len(buf) == 0:
+        return {}
+    head = np.frombuffer(buf[:16], np.int64)
+    meta_bytes, n_groups = int(head[0]), int(head[1])
+    off, coff = 16, meta_bytes
+    out = {}
+    for _ in range(n_groups):
+        h = np.frombuffer(buf[off:off + 56], np.int64)
+        off += 56
+        g, n_lines, nm = int(h[0]), int(h[1]), [int(x) for x in h[2:7]]
+        sizes = np.frombuffer(buf[off:off + 8 * sum(nm)], np.int64).copy()
+        off += 8 * sum(nm)
+        lines = np.frombuffer(buf[off:off + GROUP_LINE.itemsize * n_lines], GROUP_LINE).copy()
+        off += GROUP_LINE.itemsize * n_lines
+        us, cs, dat, k = [], [], [], 0
+        for f, m in enumerate(file_masks(lines["cls"])):
+            cs.append(sizes[k:k + nm[f]]); k += nm[f]
+            us.append(member_cuts(int(lines["text_len"][m].astype(np.int64).sum())))
+            assert us[-1].shape[0] == nm[f]
+            b = int(cs[-1].sum())
+            dat.append(bytes(buf[coff:coff + b])); coff += b
+        out[g] = GroupPart(lines, us, cs, dat)
+    return out
+
+
+class DistributedGenomeCaller:
+    """`pepper_variant call_variant -b -f -o -s [-r]` of a whole genome over all ranks of the default process group.
+
+        dgc = DistributedGenomeCaller(state, local_device, capacity_bytes)
+        totals = dgc.call_genome(bam, fasta, out_dir, "sample")   # rank 0 writes the five PEPPER_VARIANT_*.vcf.gz + .tbi
+        dgc.close()                                               # before destroy_process_group()
+
+    Every rank runs one streaming session over the groups it claims (a session takes groups of any contig), then its own VCF
+    pass over the session's device buffers with the records at its groups' boundary positions held back.  After the sessions:
+    the held-back records are all-gathered and the owner of each boundary's later group writes that boundary's line (edge pass);
+    the per-group (lines, first / last position) table is all-gathered and decides the `last_position` drops; each rank lays out
+    its lines per file and group and compresses them to BGZF members on its GPU; rank 0 gathers the members + a compact line
+    table and writes the files.  Returns the FindCandidates.py:185-189 totals on every rank.
+
+    `capacity_bytes`: the candidate records one rank's session may hold (84 bytes each); run fails when the ranks together could
+    not run every group.  `distributed=False` runs alone at world size 1."""
+
+    def __init__(self, state: dict, device: int, capacity_bytes: int, schedule: str = "dynamic", group_regions: int = 32,
+                 distributed: bool = True, caller=None):
+        import torch
+        import torch.distributed as dist
+        from .pipeline import VariantCaller
+        on = distributed and dist.is_initialized()
+        self.world = dist.get_world_size() if on else 1
+        self.rank = dist.get_rank() if on else 0
+        self._own_caller = caller is None
+        self.caller = caller if caller is not None else VariantCaller(state, device)
+        self.device_id = device
+        self.device = torch.device("cuda", device)
+        self.schedule, self.group_regions = schedule, group_regions
+        self.capacity = int(capacity_bytes)
+        self._calls = 0
+        self.phase_ms = {}
+
+    def close(self):
+        if self._own_caller:
+            self.caller.close()
+
+    # ---------------------------------------------------------------- per-rank work
+    def run_groups(self, src, claimer, params: dict, options: dict | None = None, vcf_options: dict | None = None,
+                   world: int | None = None) -> GenomeRankPart:
+        """The groups `claimer` hands out through one streaming session, the boundary records held back, and the VCF pass over
+        the rest on the device."""
+        import time
+        import torch
+        from .abi import PbCandidateColumns, regions_array, ALLELE_STRIDE
+        from .candidates import ONT_OPTIONS
+        from .frontend import FETCH_READERS
+        from .vcf import vcf_text_device, VCF_LINE
+        from ._lib import check
+        groups = src.groups(self.group_regions)
+        bnd = src.boundaries(groups)
+        part = GenomeRankPart()
+        cap = max(1, self.capacity // RECORD_BYTES)
+        t0 = time.perf_counter()
+        s = self.caller.stream(params, cap)
+
+        def stage(j):
+            g0, g1 = groups[j]
+            s.stage_device(src.take(j, g0, g1), 0, g1 - g0, g0)
+
+        def request(j):
+            src.request(j, *groups[j])
+        segments = run_claimed(s, claimer, stage, request, FETCH_READERS, cap, len(groups), world or self.world)
+        n = s.end()
+        part.groups = sorted(g for g, _ in segments)
+        part.phase_ms["sessions"] = (time.perf_counter() - t0) * 1e3
+        t0 = time.perf_counter()
+        if n > 0:
+            cols, d_probs = PbCandidateColumns(), C.c_void_p()
+            check(s.L.pb_variant_stream_columns(self.caller.enc.h, C.byref(cols), C.byref(d_probs), None), "columns")
+            group_of = np.repeat(np.arange(len(groups)), [g1 - g0 for g0, g1 in groups])
+            dev = self.device
+            pos = _device_column(cols.positions, (n,), "<i8", dev)
+            rof = _device_column(cols.region_of, (n,), "<i4", dev).long()
+            gb = torch.from_numpy(bnd).to(dev)[torch.from_numpy(group_of).to(dev)[rof]]
+            idx = torch.nonzero((pos == gb[:, 0]) | (pos == gb[:, 1])).squeeze(1)           # arrival order
+            held = np.zeros(int(idx.shape[0]), PRED_RECORD)
+            if held.shape[0]:
+                held["position"] = pos[idx].cpu().numpy()
+                held["region"] = rof[idx].cpu().numpy()
+                held["depth"] = _device_column(cols.depths, (n,), "|u1", dev)[idx].cpu().numpy()
+                held["freq"] = _device_column(cols.freqs, (n,), "|u1", dev)[idx].cpu().numpy()
+                keys = _device_column(cols.keys, (n, ALLELE_STRIDE), "|u1", dev)[idx].cpu().numpy()
+                held["key"] = np.ascontiguousarray(keys[:, :62]).view("S62")[:, 0]
+                held["probs"] = _device_column(d_probs.value, (n, 3), "<f4", dev)[idx].cpu().numpy()
+            part.held = held
+            regs = [r for g in part.groups for r in range(*groups[g])]
+            table = src.table(regs)
+            window = np.empty((src.n_regions, 2), np.int64)
+            window[:, 0] = np.where(bnd[group_of, 0] >= 0, bnd[group_of, 0] + 1, 0)
+            window[:, 1] = np.where(bnd[group_of, 1] >= 0, bnd[group_of, 1] - 1, np.iinfo(np.int64).max)
+            d_regions = torch.from_numpy(regions_array(table)[1]).to(dev)
+            d_ref = torch.from_numpy(np.ascontiguousarray(table.ref, np.uint8)).to(dev)
+            text, lines = vcf_text_device(src.names, src.contig_of, cols, d_probs.value or 0, n, d_regions.data_ptr(), d_ref.data_ptr(),
+                                          options or ONT_OPTIONS, vcf_options, self.device_id, window=window, on_device=True)
+            part.text, part.lines = text, lines.cpu().numpy().view(VCF_LINE)
+            # a line's group: the first group of its contig whose last interval ends at or after the line
+            gkey = np.array([(int(src.contig_of[g0]) << 40) | src.intervals[g1 - 1][1] for g0, g1 in groups], np.int64)
+            part.line_group = np.searchsorted(gkey, (part.lines["contig"].astype(np.int64) << 40) | part.lines["pos"], side="left")
+        part.phase_ms["vcf_pass"] = (time.perf_counter() - t0) * 1e3
+        t = self.caller.timings()
+        part.phase_ms["encoder_device"], part.phase_ms["network_device"] = t["encode_ms"], t["network_ms"]
+        return part
+
+    def edge_pass(self, part: GenomeRankPart, src, held: np.ndarray, options: dict | None = None, vcf_options: dict | None = None):
+        """For each boundary whose later group this rank ran: the VCF pass over the earlier group's held-back records at that
+        position followed by the later group's (arrival order within each) -> at most one line, the later group's first."""
+        import time
+        from .candidates import ONT_OPTIONS
+        from .synth import RegionTable
+        from .vcf import vcf_text_host
+        from .abi import ALLELE_STRIDE
+        t0 = time.perf_counter()
+        groups = src.groups(self.group_regions)
+        bnd = src.boundaries(groups)
+        group_of = np.repeat(np.arange(len(groups)), [g1 - g0 for g0, g1 in groups])
+        rg = group_of[held["region"]] if held.shape[0] else np.zeros(0, np.int64)
+        part.edges = {}
+        for g in part.groups:
+            b = int(bnd[g, 0])
+            if b < 0:
+                continue
+            sel = np.concatenate([np.flatnonzero((rg == g - 1) & (held["position"] == b)), np.flatnonzero((rg == g) & (held["position"] == b))])
+            if sel.shape[0] == 0:
+                continue
+            rec = held[sel]
+            regs = np.unique(rec["region"])
+            tab = src.table(regs)
+            keys = np.zeros((rec.shape[0], ALLELE_STRIDE), np.uint8)
+            keys[:, :62] = np.ascontiguousarray(rec["key"]).view(np.uint8).reshape(-1, 62)
+            cid = int(src.contig_of[regs[0]])
+            text, lines = vcf_text_host(src.names, np.full(regs.shape[0], cid, np.int32), rec["position"].astype(np.int64),
+                                        np.searchsorted(regs, rec["region"]).astype(np.int32), rec["depth"], rec["freq"], keys,
+                                        rec["probs"], RegionTable(tab.table[regs], tab.ref), options or ONT_OPTIONS, vcf_options)
+            if lines.shape[0]:
+                part.edges[g] = (text, lines)
+        part.phase_ms["edge"] = (time.perf_counter() - t0) * 1e3
+
+    def compress(self, part: GenomeRankPart, src, table: np.ndarray):
+        """Applies the `last_position` drops decided from the whole group table, lays out every file's lines per group on the
+        device and compresses them to BGZF members (part.meta: the compact line table and member sizes; part.comp: the
+        members, device).  Returns the totals."""
+        import time
+        import torch
+        from .vcf import VCF_LINE, file_masks, member_cuts, group_line_table, gather_lines_device, bgzf_compress_device
+        t0 = time.perf_counter()
+        groups = src.groups(self.group_regions)
+        group_contig = np.array([int(src.contig_of[g0]) for g0, _ in groups], np.int64)
+        drop = last_position_drops(table, group_contig, src.names)
+        totals = genome_totals(table, drop)
+        # one text and line table: the VCF pass's, then the edge lines
+        texts = [part.text] if part.text is not None else []
+        tabs = [part.lines] if part.lines is not None else []
+        base = int(part.text.shape[0]) if part.text is not None else 0
+        edge_row = {}
+        nrow = sum(t.shape[0] for t in tabs)
+        for g, (text, lines) in sorted(part.edges.items()):
+            t = lines.copy()
+            t["text_off"] += base
+            base += text.shape[0]
+            texts.append(torch.from_numpy(text).to(self.device)); tabs.append(t)
+            edge_row[g] = np.arange(nrow, nrow + t.shape[0]); nrow += t.shape[0]
+        all_lines = np.concatenate(tabs) if tabs else np.zeros(0, VCF_LINE)
+        sel, dst, member_off, meta = [], [], [0], [np.zeros(2, np.int64).tobytes()]
+        pay = 0
+        for g in part.groups:
+            rows = np.concatenate([edge_row.get(g, np.zeros(0, np.int64)),
+                                   np.flatnonzero(part.line_group == g) if part.lines is not None else np.zeros(0, np.int64)]).astype(np.int64)
+            if drop[g]:
+                rows = rows[1:]
+            gl = all_lines[rows]
+            nm = []
+            for m in file_masks(gl["cls"]):
+                r = rows[m]
+                ln = all_lines["text_len"][r].astype(np.int64)
+                sel.append(r); dst.append(pay + np.concatenate([[0], np.cumsum(ln)[:-1]]) if r.shape[0] else np.zeros(0, np.int64))
+                cuts = member_cuts(int(ln.sum()))
+                member_off.extend((pay + np.cumsum(cuts)).tolist())
+                pay += int(ln.sum())
+                nm.append(cuts.shape[0])
+            meta.append(np.array([g, gl.shape[0]] + nm, np.int64).tobytes())
+            meta.append(None)                        # member sizes, filled in after the compression
+            meta.append(group_line_table(gl).tobytes())
+        payload = torch.empty(max(1, pay), dtype=torch.uint8, device=self.device)
+        if pay:
+            text_all = torch.cat(texts) if len(texts) > 1 else texts[0]
+            d_lines = torch.from_numpy(all_lines.view(np.uint8).reshape(-1)).to(self.device)
+            gather_lines_device(text_all, d_lines, np.concatenate(sel), np.concatenate(dst), payload, self.device_id)
+        t1 = time.perf_counter()
+        comp, sizes = bgzf_compress_device(payload, np.array(member_off, np.int64), self.device_id)
+        torch.cuda.synchronize(self.device)
+        part.phase_ms["compress"] = (time.perf_counter() - t1) * 1e3
+        part.phase_ms["layout"] = (t1 - t0) * 1e3
+        k = 0
+        for i in range(len(meta)):
+            if meta[i] is None:
+                nm = np.frombuffer(meta[i - 1], np.int64)[2:7]
+                meta[i] = sizes[k:k + int(nm.sum())].tobytes()
+                k += int(nm.sum())
+        body = b"".join(meta)
+        body = np.frombuffer(np.array([len(body), len(part.groups)], np.int64).tobytes() + body[16:], np.uint8).copy()
+        part.meta, part.comp = body, comp
+        part.payload_bytes = pay
+        return totals
+
+    # ---------------------------------------------------------------- the collectives
+    def _all_gather_object(self, obj) -> list:
+        if self.world == 1:
+            return [obj]
+        import torch.distributed as dist
+        out = [None] * self.world
+        dist.all_gather_object(out, obj)
+        return out
+
+    def _gather_bytes(self, part: GenomeRankPart) -> list | None:
+        """Every rank's meta + members into one byte GatherBuffer (one all-gather); rank 0 gets each rank's bytes."""
+        import torch
+        mine = int(part.meta.shape[0]) + int(part.comp.shape[0])
+        cap = max(x for x in self._all_gather_object(mine))
+        buf = GatherBuffer(max(1, cap), self.world, self.rank, self.device, record=np.uint8)
+        try:
+            sl = buf.my_slice()
+            sl[:part.meta.shape[0]].copy_(torch.from_numpy(part.meta))
+            sl[part.meta.shape[0]:mine].copy_(part.comp)
+            buf.gather(mine)
+            torch.cuda.synchronize(self.device)
+            if self.rank != 0:
+                return None
+            counts = buf.meta[:, 0].cpu().numpy()
+            return [buf.records[r * buf.slice_bytes:r * buf.slice_bytes + int(counts[r])].cpu().numpy() for r in range(self.world)]
+        finally:
+            buf.release()
+
+    def call_genome(self, bam: str, fasta: str, out_dir: str, sample_name: str, region: str | None = None, exclude=(),
+                    params: dict | None = None, options: dict | None = None, vcf_options: dict | None = None,
+                    interval_size: int = 100_000, gpu_inflate: bool = True) -> tuple:
+        import time
+        from .frontend import VariantGenomeSource
+        from .synth import ont_params
+        from .vcf import write_vcfs_from_parts
+        from ._lib import PepperB200Error
+        from .abi import PB_ERR_CAPACITY
+        params = params or ont_params()
+        src = VariantGenomeSource(bam, fasta, int(params["min_snp_baseq"]), region, exclude, interval_size, self.device_id,
+                                  gpu_inflate=gpu_inflate)
+        try:
+            groups = src.groups(self.group_regions)
+            self._calls += 1
+            claimer = GroupClaimer(len(groups), self.rank, self.world, self.schedule, src.group_work(groups),
+                                   key="pb_genome_claim_%d" % self._calls)
+            part = self.run_groups(src, claimer, params, options, vcf_options)
+            t0 = time.perf_counter()
+            held = self._all_gather_object(part.held)
+            held = np.concatenate(held) if held else np.zeros(0, PRED_RECORD)
+            part.phase_ms["edge_exchange"] = (time.perf_counter() - t0) * 1e3
+            self.edge_pass(part, src, held, options, vcf_options)
+            table = sum(self._all_gather_object(group_table_rows(part, len(groups))))
+            if int(table[:, GT_RAN].sum()) != len(groups):
+                raise PepperB200Error("only %d of %d groups were run: the session capacity (%d bytes per rank) is exhausted — raise "
+                                      "`capacity_bytes`" % (int(table[:, GT_RAN].sum()), len(groups), self.capacity), PB_ERR_CAPACITY)
+            totals = self.compress(part, src, table)
+            t0 = time.perf_counter()
+            got = self._gather_bytes(part)
+            part.phase_ms["gather"] = (time.perf_counter() - t0) * 1e3
+            t0 = time.perf_counter()
+            if got is not None:
+                parts = {}
+                for data in got:
+                    parts.update(parse_rank_bytes(data))
+                write_vcfs_from_parts(out_dir, sample_name, src.fasta_contigs(), src.names,
+                                      [int(src.contig_of[g0]) for g0, _ in groups], parts)
+            part.phase_ms["write"] = (time.perf_counter() - t0) * 1e3
+            part.phase_ms["groups"] = len(part.groups)
+            self.phase_ms = {k: round(v, 2) for k, v in part.phase_ms.items()}
+            self.payload_bytes, self.member_bytes = part.payload_bytes, int(part.comp.shape[0])
+            return totals
+        finally:
+            src.close()
+
+
+def _device_column(ptr: int, shape: tuple, typestr: str, device):
+    """A torch view of a device array the library owns (valid while the session's buffers are)."""
+    import torch
+
+    class _A:
+        pass
+    a = _A()
+    a.__cuda_array_interface__ = dict(shape=shape, typestr=typestr, data=(int(ptr), False), version=3)
+    return torch.as_tensor(a, device=device)

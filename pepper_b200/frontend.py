@@ -405,6 +405,106 @@ class VariantFileSource(_FromFiles):
         super().close()
 
 
+def genome_plan(fasta_contigs: list[tuple[str, int]], bam_contigs: list[str], region: str | None = None, exclude=(),
+                interval_size: int = 100_000):
+    """The job of a whole-genome call: the contigs of variant_job, each tiled with variant_intervals(start, end, interval_size),
+    the intervals laid out contig after contig.  Returns (contig names, intervals, first interval of each contig + the total)."""
+    job = variant_job(fasta_contigs, bam_contigs, region, exclude)
+    intervals, first = [], []
+    for _, s, e in job:
+        first.append(len(intervals))
+        intervals.extend(variant_intervals(s, e, interval_size))
+    first.append(len(intervals))
+    return [c for c, _, _ in job], intervals, first
+
+
+def group_boundaries(intervals: list[tuple[int, int]], first: list[int], groups: list[tuple[int, int]]) -> np.ndarray:
+    """[n_groups, 2] (left, right) boundary positions of each group, -1 where there is none: the start of its first interval
+    unless that is the first of its contig, the end of its last interval unless that is the last of its contig.  Group g's right
+    boundary is group g+1's left boundary; both groups' intervals emit candidates at that shared position."""
+    firsts = set(first[:-1])
+    lasts = {f - 1 for f in first[1:]}
+    return np.array([[intervals[g0][0] if g0 not in firsts else -1, intervals[g1 - 1][1] if g1 - 1 not in lasts else -1]
+                     for g0, g1 in groups], np.int64).reshape(-1, 2)
+
+
+class VariantGenomeSource(_FromFiles):
+    """The read source of dist.DistributedGenomeCaller: every contig of variant_job (the contigs call_genome processes, with the
+    same `region` / `exclude` handling), each tiled with variant_intervals(start, end, interval_size), the intervals laid out
+    contig after contig.  Groups (`groups`) are runs of whole intervals that never cross a contig; `request` / `take` fetch and
+    trim a group's reads as VariantFileSource does.  Contig id k is the k-th contig of the job (call_genome's numbering)."""
+
+    def __init__(self, bam_path: str, fasta_path: str, min_snp_baseq: int, region: str | None = None, exclude=(),
+                 interval_size: int = 100_000, device: int = 0, threads: int = 0, gpu_inflate: bool = True,
+                 include_supplementary: bool = False, min_mapq: int = 0, downsample_rate: float = 1.0,
+                 max_reads: int = VARIANT_MAX_READS, host_share: float | None = None):
+        from concurrent.futures import ThreadPoolExecutor
+        super().__init__(bam_path, fasta_path, device, threads, gpu_inflate, host_share)
+        self.names, self.intervals, self._first = genome_plan(self.fasta_contigs(), self.bam.get_chromosome_sequence_names(), region,
+                                                             exclude, interval_size)
+        self.contig_of = np.repeat(np.arange(len(self.names), dtype=np.int32), np.diff(self._first))
+        self._filters = (int(min_snp_baseq), include_supplementary, min_mapq, max_reads, downsample_rate)
+        self._ring = self._readers(FETCH_READERS)
+        self._pool = ThreadPoolExecutor(max_workers=FETCH_WORKERS)
+        self._futs, self._issued = {}, 0
+
+    def fasta_contigs(self) -> list[tuple[str, int]]:
+        return [(c, self.fasta.get_chromosome_sequence_length(c)) for c in self.fasta.get_chromosome_names()]
+
+    @property
+    def n_regions(self) -> int:
+        return len(self.intervals)
+
+    def regions_per_contig(self) -> list[int]:
+        return [self._first[k + 1] - self._first[k] for k in range(len(self.names))]
+
+    def groups(self, group_regions: int = 32) -> list[tuple[int, int]]:
+        from .dist import plan_polish_groups
+        return plan_polish_groups(self.regions_per_contig(), group_regions)
+
+    def boundaries(self, groups: list[tuple[int, int]]) -> np.ndarray:
+        return group_boundaries(self.intervals, self._first, groups)
+
+    def group_work(self, groups: list[tuple[int, int]]) -> np.ndarray:
+        """Genomic bases per group: the work estimate the static schedule balances."""
+        return np.array([self.intervals[g1 - 1][1] - self.intervals[g0][0] + 1 for g0, g1 in groups], dtype=np.int64)
+
+    def table(self, regions) -> RegionTable:
+        """The region table + reference of the given region ids, in rows as call_genome's genome_table builds them (the reference
+        offsets point into one string); the other rows are zero."""
+        rows = np.zeros((self.n_regions, 8), np.int64)
+        refs, base = [], 0
+        by_contig = {}
+        for r in sorted(int(x) for x in regions):
+            by_contig.setdefault(int(self.contig_of[r]), []).append(r)
+        for k, rs in by_contig.items():
+            rr, spans = [], []
+            for r in rs:
+                a, b = self.intervals[r]
+                s, e = max(0, a - REGION_SAFE_BASES), b + REGION_SAFE_BASES
+                rr.append([s, e, a, b, 0, 0, 0, 0]); spans.append((s, e + 1))
+            t = self._ref_table(self.names[k], rr, spans)
+            t.table[:, 4] += base
+            rows[rs] = t.table
+            refs.append(t.ref); base += t.ref.shape[0]
+        return RegionTable(rows, np.concatenate(refs) if refs else np.zeros(1, np.uint8))
+
+    def request(self, key, g0: int, g1: int) -> None:
+        reader = self._ring[self._issued % FETCH_READERS]
+        self._issued += 1
+        self._futs[key] = self._pool.submit(self._fetch, reader, self.names[self.contig_of[g0]], *self._group_span(self.intervals[g0:g1]))
+
+    def take(self, key, g0: int, g1: int) -> FetchedReads:
+        view = self._futs.pop(key).result()            # a Future re-raises the worker's exception (bad contig, corrupt block) here
+        return self._trim_variant(view, self.names[self.contig_of[g0]], self.intervals[g0:g1], *self._filters)
+
+    def close(self):
+        if getattr(self, "_pool", None) is not None:
+            self._pool.shutdown(wait=True)
+            self._pool = None
+        super().close()
+
+
 class PolishFromFiles(_FromFiles):
     """polish's make_images (with read realignment) + call_consensus for a list of regions of one contig."""
 

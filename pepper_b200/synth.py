@@ -197,13 +197,21 @@ def _ascii_to_code(ref: np.ndarray) -> np.ndarray:
 
 def simulate_region_reads(ref: np.ndarray, ref_start: int, coverage: float, platform: Platform, seed: int,
                           p_soft_tail: float = 0.02, p_n_base: float = 1e-4, p_low_mapq: float = 0.01,
-                          hp_mask: np.ndarray | None = None) -> ReadBatch:
+                          hp_mask: np.ndarray | None = None, truth=()) -> ReadBatch:
     """Reads over a padded region whose reference string is `ref` (positions ref_start..ref_start+len-1),
-    each already trimmed to the region as get_reads would (first op M, inside [ref_start, ref_end])."""
+    each already trimmed to the region as get_reads would (first op M, inside [ref_start, ref_end]).  `truth`: variants placed
+    on top of the random ones, (position, "snp" / "del" / "ins", alt base or length, haplotypes); the random draws are
+    unchanged by it."""
     rng = np.random.default_rng(seed)
     L = ref.shape[0]
     refc = _ascii_to_code(ref)
     hap_snp, hap_del, hap_ins = _truth_variants(rng, ref)
+    for p, kind, v, haps in truth:
+        for h in haps:
+            if kind == "snp":
+                hap_snp[h, p - ref_start] = CODE_OF[v]
+            else:
+                (hap_del if kind == "del" else hap_ins)[h, p - ref_start] = int(v)
     if hp_mask is None:
         same = np.zeros(L, dtype=bool)
         same[1:] = ref[1:] == ref[:-1]
@@ -455,12 +463,12 @@ def make_records(records: list[dict]) -> RecordBatch:
 
 
 def simulate_contig_records(contig_len: int, coverage: float, platform: Platform, seed: int, contig_start: int = 0,
-                            p_clip_head: float = 0.3, p_hard: float = 0.05, p_filtered: float = 0.06):
+                            p_clip_head: float = 0.3, p_hard: float = 0.05, p_filtered: float = 0.06, truth=()):
     """Whole-contig alignment records: the read model of simulate_region_reads over the full contig, then decorated the
     way an aligner's output is — leading soft / hard clips, trailing hard clips, SAM FLAG bits (reverse, secondary,
     supplementary, duplicate, QC-fail, unmapped).  Returns (RecordBatch, genome uint8 ASCII)."""
     genome = make_reference(contig_len, seed)
-    b = simulate_region_reads(genome, contig_start, coverage, platform, seed * 7919 + 13)
+    b = simulate_region_reads(genome, contig_start, coverage, platform, seed * 7919 + 13, truth=truth)
     rng = np.random.default_rng(seed + 991)
     codes = b.codes()
     pos, flag, code_l, qual_l, cig_l = [], [], [], [], []

@@ -168,7 +168,8 @@ class PbVcfOptions(C.Structure):
 
 
 class PbVcfJob(C.Structure):
-    _fields_ = [("contig_of_region", C.c_void_p), ("names", C.c_void_p), ("name_off", C.c_void_p), ("vaf_table", C.c_void_p)]
+    _fields_ = [("contig_of_region", C.c_void_p), ("names", C.c_void_p), ("name_off", C.c_void_p), ("vaf_table", C.c_void_p),
+                ("window", C.c_void_p)]
 
 
 # pb_vcf_line_t; cls: 0 = pepper, 1 = variant-calling SNP, 2 = variant-calling indel
@@ -244,9 +245,12 @@ def vcf_text_host(names: list[str], contig_of_region, positions, region_of, dept
 
 
 def vcf_text_device(names: list[str], contig_of_region, cols, d_probs: int, n: int, d_regions: int, d_ref: int, options: dict,
-                    vcf_opts: dict | None = None, device: int = 0, stream: int = 0):
+                    vcf_opts: dict | None = None, device: int = 0, stream: int = 0, window: np.ndarray | None = None,
+                    on_device: bool = False):
     """pb_variant_vcf_device over records already in HBM (`cols`: abi.PbCandidateColumns of device pointers) -> (text uint8, line
-    table) on the host: only the VCF text and its line table leave the GPU."""
+    table) on the host: only the VCF text and its line table leave the GPU.  `window` [n_regions, 2]: the positions [lo, hi]
+    each region's records may form sites at (None: all).  `on_device`: the text and the line table stay on the device (uint8
+    tensors)."""
     import torch
     from .candidates import PbCandidateOptions
     from .abi import PbCandidateColumns
@@ -258,6 +262,8 @@ def vcf_text_device(names: list[str], contig_of_region, cols, d_probs: int, n: i
     dev = torch.device("cuda", device)
     nm, off = _names_blob(names)
     keep = [torch.from_numpy(x).to(dev) for x in (np.ascontiguousarray(contig_of_region, np.int32), nm, off, vaf_table().reshape(-1))]
+    if window is not None:
+        keep.append(torch.from_numpy(np.ascontiguousarray(window, np.int64).reshape(-1)).to(dev))
     job = PbVcfJob(*(t.data_ptr() for t in keep))
     so, vo = PbCandidateOptions(**options), vcf_options(vcf_opts or VCF_OPTIONS_ONT)
     text_cap, lines_cap = max(1, 160 * n), max(1, n)
@@ -272,7 +278,8 @@ def vcf_text_device(names: list[str], contig_of_region, cols, d_probs: int, n: i
             text_cap, lines_cap = int(nt.value), int(nl.value)
             continue
         _lib.check(rc, "pb_variant_vcf_device")
-        return (text[:nt.value].cpu().numpy(), lines[:nl.value * VCF_LINE.itemsize].cpu().numpy().view(VCF_LINE))
+        text, lines = text[:nt.value], lines[:nl.value * VCF_LINE.itemsize]
+        return (text, lines) if on_device else (text.cpu().numpy(), lines.cpu().numpy().view(VCF_LINE))
 
 
 def host_tail_text(records: list[dict], contig_id: int):
@@ -355,18 +362,59 @@ def _tabix(names: list[str], tids: np.ndarray, beg: np.ndarray, end: np.ndarray,
            blk_u: np.ndarray, blk_c: np.ndarray, eof_c: int, total_u: int) -> bytes:
     """TBI of a VCF (format 2, col_seq 1, col_beg 2, col_end 0, meta '#'): the per-reference bins / chunks / 16 kb linear index
     are those of a BAI (synth_files._bai_bytes) over [pos, pos + len(REF)) and the lines' virtual offsets."""
-    from .synth_files import _bai_bytes
+    blk_u, blk_c = np.asarray(blk_u, np.int64), np.asarray(blk_c, np.int64)
 
-    u = np.concatenate([ustart, uend]).astype(np.int64)
-    k = np.maximum(np.searchsorted(blk_u, u, side="right") - 1, 0)
-    v = np.where(u >= total_u, np.int64(eof_c) << 16, (blk_c[k] << 16) | (u - blk_u[k]))
-    voff = dict(zip(u.tolist(), v.tolist())).__getitem__          # every line's virtual offsets from one searchsorted
-    spans = {}
-    for t, b, e, us, ue in zip(tids.tolist(), beg.tolist(), end.tolist(), ustart.tolist(), uend.tolist()):
-        spans.setdefault(t, []).append((b, e, us, ue))
+    def voff(u):
+        u = np.asarray(u, np.int64)
+        k = np.maximum(np.searchsorted(blk_u, u, side="right") - 1, 0)
+        return np.where(u >= total_u, np.int64(eof_c) << 16, (blk_c[k] << 16) | (u - blk_u[k])).astype(np.uint64)
+    tids = np.asarray(tids, np.int64)
+    beg, end = np.asarray(beg, np.int64), np.asarray(end, np.int64)
+    vb, ve = voff(ustart), voff(uend)
     nm = b"".join(n.encode() + b"\0" for n in names)
-    head = b"TBI\x01" + struct.pack("<8i", len(names), 2, 1, 2, 0, ord("#"), 0, len(nm)) + nm
-    return head + _bai_bytes(len(names), spans, voff)[8:]
+    out = [b"TBI\x01" + struct.pack("<8i", len(names), 2, 1, 2, 0, ord("#"), 0, len(nm)) + nm]
+    for t in range(len(names)):
+        sel = np.flatnonzero(tids == t)
+        out.append(_index_reference(beg[sel], end[sel], vb[sel], ve[sel]))
+    return b"".join(out)
+
+
+def _index_reference(beg: np.ndarray, end: np.ndarray, vb: np.ndarray, ve: np.ndarray) -> bytes:
+    """One reference's bins, chunks, pseudo-bin and 16 kb linear index: the bytes synth_files._bai_bytes writes for the spans
+    (beg, end) with virtual offsets [vb, ve), lines in file order.  A chunk is a run of consecutive lines of one bin (the lines
+    lie back to back, so _bai_bytes merges exactly those); a window's linear offset is the first line that covers it, and a
+    window no line covers takes the previous window's."""
+    from .synth_files import _reg2bin_v
+    n = beg.shape[0]
+    if n == 0:
+        return struct.pack("<ii", 0, 0)
+    bins = _reg2bin_v(beg, end)
+    brk = np.flatnonzero(bins[1:] != bins[:-1]) + 1
+    first, last = np.concatenate([[0], brk]), np.concatenate([brk, [n]]) - 1
+    cbin, cvb, cve = bins[first], vb[first], ve[last]
+    o = np.argsort(cbin, kind="stable")
+    cbin, cvb, cve = cbin[o], cvb[o], cve[o]
+    ub, ufirst, cnt = np.unique(cbin, return_index=True, return_counts=True)
+    nb, nc = ub.shape[0], cbin.shape[0]
+    words = np.zeros(2 * nb + 4 * nc, np.uint32)                 # per bin: bin, n_chunk, then (beg, end) as uint64 pairs
+    bstart = 2 * np.arange(nb) + 4 * ufirst
+    words[bstart], words[bstart + 1] = ub, cnt
+    cpos = 2 * (np.repeat(np.arange(nb), cnt) + 1) + 4 * np.arange(nc)
+    lo32 = np.uint64(0xffffffff)
+    for k, v in enumerate((cvb & lo32, cvb >> np.uint64(32), cve & lo32, cve >> np.uint64(32))):
+        words[cpos + k] = v
+    meta = struct.pack("<Ii", 37450, 2) + struct.pack("<QQQQ", int(vb[0]), int(ve[-1]), n, 0)
+    wa, wb = beg >> 14, (end - 1) >> 14
+    n_win = int(wb.max()) + 1
+    span = wb - wa + 1
+    line = np.repeat(np.arange(n), span)
+    win = np.repeat(wa, span) + np.arange(line.shape[0]) - np.repeat(np.cumsum(span) - span, span)
+    none = np.iinfo(np.uint64).max
+    lin = np.full(n_win, none, np.uint64)
+    np.minimum.at(lin, win, vb[line])
+    idx = np.maximum.accumulate(np.where(lin != none, np.arange(n_win), -1))
+    lin = np.where(idx >= 0, lin[np.maximum(idx, 0)], np.uint64(0)).astype("<u8")
+    return (struct.pack("<i", nb + 1) + words.astype("<u4").tobytes() + meta + struct.pack("<i", n_win) + lin.tobytes())
 
 
 def write_vcfs(out_dir: str, sample_name: str, fasta_contigs: list[tuple[str, int]], names: list[str], text: np.ndarray,
@@ -397,3 +445,156 @@ def write_vcfs(out_dir: str, sample_name: str, fasta_contigs: list[tuple[str, in
             with open(path + ".tbi", "wb") as f:
                 f.write(_bgzf(tbi, pool)[0])
     return tuple(int(m.sum()) for m in masks)
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# Whole-genome output from BGZF members compressed elsewhere (each rank's GPU): the files are the header member, then every
+# group's members in lexical contig order and group order, then the EOF block; only the members and a compact line table reach
+# the writer.
+
+# what the writer needs of a line: its position, REF length, class and length (its offset is the sum of the lengths before it)
+GROUP_LINE = np.dtype([("pos", "<i8"), ("ref_len", "<i4"), ("cls", "<i4"), ("text_len", "<i4"), ("pad", "<i4")])
+
+
+def file_masks(cls: np.ndarray) -> tuple:
+    """The lines each of VCF_FILES takes, by class (write_vcfs)."""
+    return (np.ones(cls.shape[0], bool), cls == CLASS_PEPPER, cls != CLASS_PEPPER, cls == CLASS_VC_SNP, cls == CLASS_VC_INDEL)
+
+
+def member_cuts(stream_bytes: int, payload: int = BGZF_PAYLOAD) -> np.ndarray:
+    """Payload sizes of the members one group stream is cut into (every member but the last is full; a member may end
+    mid-line)."""
+    n = -(-int(stream_bytes) // payload)
+    cuts = np.full(n, payload, np.int64)
+    if n:
+        cuts[-1] = int(stream_bytes) - payload * (n - 1)
+    return cuts
+
+
+class GroupPart:
+    """One group's share of the five files: its lines (GROUP_LINE, in file order) and, per file, the payload and compressed
+    sizes of its members and their bytes."""
+
+    def __init__(self, lines: np.ndarray, usizes: list, csizes: list, data: list):
+        self.lines, self.usizes, self.csizes, self.data = lines, usizes, csizes, data
+
+
+def group_line_table(lines: np.ndarray) -> np.ndarray:
+    out = np.zeros(lines.shape[0], GROUP_LINE)
+    for k in ("pos", "ref_len", "cls", "text_len"):
+        out[k] = lines[k]
+    return out
+
+
+def host_group_part(text: np.ndarray, lines: np.ndarray, payload: int = BGZF_PAYLOAD, level: int = 1) -> GroupPart:
+    """A GroupPart compressed on the host with zlib (the reference for the GPU compressor's parts)."""
+    from .synth_files import _bgzf_block
+    us, cs, data = [], [], []
+    for m in file_masks(lines["cls"]):
+        body = _gather(text, lines[m])
+        cuts = member_cuts(len(body), payload)
+        starts = np.concatenate([[0], np.cumsum(cuts)])
+        blocks = [_bgzf_block(body[a:b], level) for a, b in zip(starts[:-1].tolist(), starts[1:].tolist())]
+        us.append(cuts); cs.append(np.array([len(b) for b in blocks], np.int64)); data.append(b"".join(blocks))
+    return GroupPart(group_line_table(lines), us, cs, data)
+
+
+def write_vcfs_from_parts(out_dir: str, sample_name: str, fasta_contigs: list[tuple[str, int]], names: list[str],
+                          group_contig: list[int], parts: dict) -> None:
+    """The five bgzipped, tabix-indexed VCFs from compressed group parts: `parts` {group id: GroupPart}, group g of contig
+    names[group_contig[g]]; the lines are final (the last_position drop already applied).  Same files as write_vcfs over the
+    same lines, up to the DEFLATE bytes of the members."""
+    import os
+    from concurrent.futures import ThreadPoolExecutor
+    from .synth_files import BGZF_EOF
+    os.makedirs(out_dir, exist_ok=True)
+    head = vcf_header(sample_name, fasta_contigs).encode()
+    lex = {c: i for i, c in enumerate(sorted(range(len(names)), key=lambda i: names[i]))}
+    order = sorted(parts, key=lambda g: (lex[group_contig[g]], g))
+    with ThreadPoolExecutor(max_workers=8) as pool:
+        hgz, hu, hc = _bgzf(head, pool, 1)
+        hgz = hgz[:-len(BGZF_EOF)]
+        for f, name in enumerate(VCF_FILES):
+            chunks, blk_u, blk_c = [hgz], [hu], [hc[:-1]]
+            u, c = len(head), len(hgz)
+            tids, beg, end, ulen, seen = [], [], [], [], {}
+            for g in order:
+                p = parts[g]
+                sel = p.lines[file_masks(p.lines["cls"])[f]]
+                if p.usizes[f].shape[0]:
+                    blk_u.append(u + np.concatenate([[0], np.cumsum(p.usizes[f])[:-1]]))
+                    blk_c.append(c + np.concatenate([[0], np.cumsum(p.csizes[f])[:-1]]))
+                    chunks.append(p.data[f])
+                    u += int(p.usizes[f].sum()); c += int(p.csizes[f].sum())
+                if sel.shape[0]:
+                    tids.append(np.full(sel.shape[0], seen.setdefault(group_contig[g], len(seen)), np.int64))
+                    beg.append(sel["pos"]); end.append(sel["pos"] + sel["ref_len"]); ulen.append(sel["text_len"].astype(np.int64))
+            path = os.path.join(out_dir, name + ".vcf.gz")
+            with open(path, "wb") as fh:
+                fh.write(b"".join(chunks) + BGZF_EOF)
+            cat = (lambda a, dt: np.concatenate(a) if a else np.zeros(0, dt))     # noqa: E731
+            ul = cat(ulen, np.int64)
+            us = len(head) + np.concatenate([[0], np.cumsum(ul)])
+            tbi = _tabix([names[k] for k in seen], cat(tids, np.int64), cat(beg, np.int64), cat(end, np.int64), us[:-1], us[1:],
+                         np.concatenate(blk_u), np.concatenate(blk_c), c, u)
+            with open(path + ".tbi", "wb") as fh:
+                fh.write(_bgzf(tbi, pool)[0])
+
+
+def bgzf_compress_host(payload: np.ndarray, member_off: np.ndarray) -> tuple[bytes, np.ndarray]:
+    """pb_bgzf_compress_host: payload bytes [member_off[k], member_off[k + 1]) -> BGZF member k; returns (members back to back,
+    bytes of each member)."""
+    _lib.require_gpu()
+    L = _lib.lib()
+    vp = C.c_void_p
+    L.pb_bgzf_compress_host.argtypes = [vp, vp, C.c_int64, vp, C.c_int64, vp, C.POINTER(C.c_int64), vp]
+    payload = np.ascontiguousarray(payload, np.uint8)
+    off = np.ascontiguousarray(member_off, np.int64)
+    n = off.shape[0] - 1
+    sizes = np.zeros(max(1, n), np.int64)
+    cap = max(64, int(off[-1] - off[0]) // 2 + 64 * n)
+    while True:
+        out = np.empty(cap, np.uint8)
+        total = C.c_int64(0)
+        rc = L.pb_bgzf_compress_host(payload.ctypes.data, off.ctypes.data, n, out.ctypes.data, cap, sizes.ctypes.data, C.byref(total), None)
+        if rc == PB_ERR_CAPACITY:
+            cap = int(total.value)
+            continue
+        _lib.check(rc, "pb_bgzf_compress_host")
+        return out[:total.value].tobytes(), sizes[:n].copy()
+
+
+def bgzf_compress_device(d_payload, member_off: np.ndarray, device: int = 0, stream: int = 0):
+    """pb_bgzf_compress_device over a device byte tensor -> (members back to back as a device uint8 tensor, bytes of each
+    member)."""
+    import torch
+    L = _lib.lib()
+    vp = C.c_void_p
+    L.pb_bgzf_compress_device.argtypes = [vp, vp, C.c_int64, vp, C.c_int64, vp, C.POINTER(C.c_int64), vp]
+    off = np.ascontiguousarray(member_off, np.int64)
+    n = off.shape[0] - 1
+    sizes = np.zeros(max(1, n), np.int64)
+    cap = max(64, int(off[-1] - off[0]) // 4 + 64 * n)
+    while True:
+        out = torch.empty(cap, dtype=torch.uint8, device=torch.device("cuda", device))
+        total = C.c_int64(0)
+        rc = L.pb_bgzf_compress_device(vp(d_payload.data_ptr()), off.ctypes.data, n, vp(out.data_ptr()), cap, sizes.ctypes.data,
+                                       C.byref(total), vp(stream))
+        if rc == PB_ERR_CAPACITY:
+            cap = int(total.value)
+            continue
+        _lib.check(rc, "pb_bgzf_compress_device")
+        return out[:total.value], sizes[:n].copy()
+
+
+def gather_lines_device(d_text, d_lines, sel: np.ndarray, dst: np.ndarray, out, device: int = 0, stream: int = 0) -> None:
+    """pb_vcf_gather_lines_device: line sel[i] of the device line table -> out[dst[i]:], on the device."""
+    import torch
+    L = _lib.lib()
+    vp = C.c_void_p
+    L.pb_vcf_gather_lines_device.argtypes = [vp, vp, vp, vp, C.c_int64, vp, vp]
+    dev = torch.device("cuda", device)
+    s = torch.from_numpy(np.ascontiguousarray(sel, np.int64)).to(dev)
+    d = torch.from_numpy(np.ascontiguousarray(dst, np.int64)).to(dev)
+    _lib.check(L.pb_vcf_gather_lines_device(vp(d_text.data_ptr()), vp(d_lines.data_ptr()), vp(s.data_ptr()), vp(d.data_ptr()),
+                                            int(s.shape[0]), vp(out.data_ptr()), vp(stream)), "pb_vcf_gather_lines_device")

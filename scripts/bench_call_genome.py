@@ -4,7 +4,12 @@ the lexical order of the VCF) -> VariantFromFiles.call_genome -> the five bgzipp
 The same job then goes through the host tail (call_stream -> D2H of the candidate columns -> find_site_records, i.e. the CUDA
 selection + the array / Python site assembly -> format_vcf_line -> the same writer); both sets of files are compared byte for byte
 after decompression.  Prints one JSON line.  Default size: 64 Mb in total (chr20), 20x ONT.
-    python scripts/bench_call_genome.py [--total-mb 64] [--coverage 20]"""
+    python scripts/bench_call_genome.py [--total-mb 64] [--coverage 20]
+
+Under torchrun the ranks run dist.DistributedGenomeCaller on the same job instead (rank 0 simulates the files into a directory
+every rank reads): rank 0 prints the JSON line with each stage's maximum over the ranks, and `verified` compares the decompressed
+files with a one-GPU call_genome run on rank 0 outside the timed window.
+    torchrun --nproc-per-node N scripts/bench_call_genome.py [--total-mb 64]"""
 import argparse
 import gzip
 import json
@@ -101,5 +106,82 @@ def main():
         notes="one GPU: no gather (gather ms null); vcf_pass = host wall around the synchronous device VCF pass, uploads included")))
 
 
+def main_distributed():
+    import torch
+    import torch.distributed as dist
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--total-mb", type=float, default=64.0)
+    ap.add_argument("--coverage", type=float, default=20.0)
+    ap.add_argument("--seed", type=int, default=41)
+    ap.add_argument("--dir", default=os.path.join(tempfile.gettempdir(), "bench_call_genome_dist"))
+    a = ap.parse_args()
+    rank, local = int(os.environ["RANK"]), int(os.environ.get("LOCAL_RANK", 0))
+    torch.cuda.set_device(local)
+    dist.init_process_group("nccl", device_id=torch.device("cuda", local))
+    world = dist.get_world_size()
+    from oracle import nets
+    from pepper_b200 import synth, synth_files, _lib
+    from pepper_b200.dist import DistributedGenomeCaller
+    from pepper_b200.frontend import VariantFromFiles
+    from pepper_b200.vcf import VCF_FILES
+    _lib.require_gpu()
+    shares = [("chr1", 0.34), ("chr2", 0.27), ("chr10", 0.22), ("chrX", 0.17)]
+    sizes = [int(a.total_mb * 1e6 * f) for _, f in shares]
+    bam, fa = os.path.join(a.dir, "g.bam"), os.path.join(a.dir, "g.fa")
+    if rank == 0:
+        os.makedirs(a.dir, exist_ok=True)
+        recs, fasta = {}, []
+        with ProcessPoolExecutor(max_workers=len(shares)) as pool:
+            futs = [pool.submit(synth.simulate_contig_records, n, a.coverage, synth.ONT, a.seed + tid) for tid, n in enumerate(sizes)]
+            for tid, ((c, _), fut) in enumerate(zip(shares, futs)):
+                recs[tid], g = fut.result()
+                fasta.append((c, g))
+        synth_files.write_bam(bam, [(c, n) for (c, _), n in zip(shares, sizes)], recs)
+        synth_files.write_fasta(fa, fasta)
+        log("files written")
+    dist.barrier()
+    state, params = nets.make_variant_weights(0), synth.ont_params()
+    # session room: about one candidate per 15 genomic bases of this rank's share (84 bytes each)
+    dgc = DistributedGenomeCaller(state, local, 84 * (sum(sizes) // 15 // world + (1 << 16)), "dynamic")
+    dgc.call_genome(bam, fa, os.path.join(a.dir, "warm"), "sample", region="chr2:0-2000000", params=params)
+    dist.barrier()
+    t0 = time.perf_counter()
+    totals = dgc.call_genome(bam, fa, os.path.join(a.dir, "dist"), "sample", params=params)
+    dist.barrier()
+    wall = time.perf_counter() - t0
+    phases = [None] * world
+    dist.all_gather_object(phases, dgc.phase_ms)
+    extra = [None] * world
+    dist.all_gather_object(extra, (dgc.payload_bytes, dgc.member_bytes))
+    dgc.close()
+    if rank == 0:
+        card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                              text=True).stdout.strip().splitlines()[0]
+        with VariantFromFiles(bam, fa, state) as vf:
+            t1 = time.perf_counter()
+            want = vf.call_genome(os.path.join(a.dir, "one"), "sample", params=params)
+            one_wall = time.perf_counter() - t1
+            one_prof = dict(vf.last_genome_profile)
+        same = want == totals and all(
+            gzip.decompress(open(os.path.join(a.dir, "dist", f + ".vcf.gz"), "rb").read())
+            == gzip.decompress(open(os.path.join(a.dir, "one", f + ".vcf.gz"), "rb").read()) for f in VCF_FILES)
+        stage = lambda k: round(max(p.get(k, 0.0) for p in phases), 2)      # noqa: E731
+        pay, comp = sum(x for x, _ in extra), sum(y for _, y in extra)
+        print(json.dumps(dict(
+            metric="call_genome_distributed", value=sum(sizes) / wall, unit="genomic bases/s", wall_s=round(wall, 3), gpus=world,
+            genomic_bases=sum(sizes), coverage=a.coverage, totals=totals,
+            stage_ms=dict(sessions=stage("sessions"), vcf_pass=stage("vcf_pass"), edge_exchange=stage("edge_exchange"),
+                          edge_pass=stage("edge"), layout=stage("layout"), compression=stage("compress"), gather=stage("gather"),
+                          index_and_write=stage("write"), encoder_device=stage("encoder_device"), network_device=stage("network_device")),
+            compressor=dict(payload_bytes=pay, member_bytes=comp, ratio=round(pay / max(1, comp), 2),
+                            gb_per_s=round(pay / max(1e-9, stage("compress") / 1e3) / 1e9, 3)),
+            one_gpu_call_genome=dict(wall_s=round(one_wall, 3), stage_ms=one_prof),
+            verified=bool(same), card=card)))
+    dist.destroy_process_group()
+
+
 if __name__ == "__main__":
-    main()
+    if "WORLD_SIZE" in os.environ and "RANK" in os.environ:
+        main_distributed()
+    else:
+        main()

@@ -22,5 +22,6 @@ for tool in memcheck racecheck; do
     run realign $tool tests/test_realign_edges_gpu.py -k "reject or (match_port and 8)"                # k_sw16<8>, k_banded
     run stitch_sink $tool tests/test_polish_assembly_gpu.py -k "stitch_sink"                           # k_stitch_sink
     run vcf $tool tests/test_genome_vcf_gpu.py -k "vcf_host"                                         # k_site_sizes, k_site_write
+    run bgzf_deflate $tool tests/test_genome_dist_gpu.py -k "compressor"                             # k_bgzf_deflate, k_bgzf_compact
 done
 cat "$OUT/sanitizer_summary.txt"
