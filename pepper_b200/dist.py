@@ -190,18 +190,8 @@ class GatherBuffer:
         ranks reported their group segments — so no host-side re-ordering pass is needed).  The returned array is a view of
         that buffer (valid until the next to_host)."""
         import torch
-        meta = self.meta.cpu().numpy()
-        counts = [int(meta[r, 0]) for r in range(self.world)]
+        counts, segs = self._parse_meta()
         total = sum(counts)
-        segs = []                                              # (group id, source record index in the gather buffer, count)
-        for r in range(self.world):
-            off = r * self.capacity
-            for i in range(self.max_groups):
-                g, k = int(meta[r, 1 + 2 * i]), int(meta[r, 2 + 2 * i])
-                if g < 0:
-                    break
-                segs.append((g, off, k))
-                off += k
         by_segment = order and bool(segs) and sum(k for _, _, k in segs) == total
         if by_segment:
             segs.sort()
@@ -234,15 +224,22 @@ class GatherBuffer:
 
     def segments(self) -> list[tuple[int, int]]:
         """(group id, records) of every group every rank ran, sorted by group id (after gather_meta)."""
+        return sorted((g, k) for g, _, k in self._parse_meta()[1])
+
+    def _parse_meta(self) -> tuple[list[int], list[tuple[int, int, int]]]:
+        """The gathered meta table on the host: every rank's record count, and (group id, source record index in the gather
+        buffer, records) of every group every rank ran, rank-major in run order."""
         meta = self.meta.cpu().numpy()
-        out = []
+        counts, segs = [int(meta[r, 0]) for r in range(self.world)], []
         for r in range(self.world):
+            off = r * self.capacity
             for i in range(self.max_groups):
                 g, k = int(meta[r, 1 + 2 * i]), int(meta[r, 2 + 2 * i])
                 if g < 0:
                     break
-                out.append((g, k))
-        return sorted(out)
+                segs.append((g, off, k))
+                off += k
+        return counts, segs
 
     def release(self):
         """Drops the NCCL-registered pool BEFORE the process group goes away (a registered MemPool destroyed after
@@ -317,44 +314,116 @@ def run_claimed(s, claimer: GroupClaimer, stage, request, depth: int, capacity: 
     return segments
 
 
-class DistributedVariantCaller:
-    """make_images + run_inference of ONE job (a region list every rank can read) over all ranks of the default process group.
+def check_groups_ran(done: int, n_job: int, capacity: str, option: str) -> None:
+    """Raises PB_ERR_CAPACITY unless the ranks together ran all `n_job` groups.  Under any schedule and world size, run_claimed
+    stops claiming when a rank's `capacity` (named in the message, with the `option` that raises it) could not hold another
+    group, so the groups it did not run would otherwise be missing from the result without a word."""
+    if done != n_job:
+        from ._lib import PepperB200Error
+        from .abi import PB_ERR_CAPACITY
+        raise PepperB200Error("only %d of %d groups were run: %s is exhausted — raise `%s`" % (done, n_job, capacity, option),
+                              PB_ERR_CAPACITY)
 
-        dvc = DistributedVariantCaller(state, local_device, capacity)
-        dvc.run(source, regions, params)        # source: abi.HostReads (pinned host buffers), pipeline.DeviceReads, or
-                                                # frontend.VariantFileSource (BAM + FASTA every rank opens; regions=None)
-        records = dvc.buffer.to_host()          # every rank holds the whole job's records after the gather
-    """
 
-    def __init__(self, state: dict, device: int, capacity: int, schedule: str = "dynamic", group_regions: int = 32):
+class _RankDriver:
+    """What the distributed drivers share: this process's rank in the default process group (world size 1 with
+    `distributed=False` or without a process group), the caller it runs (closed with the driver unless it was given), a claim
+    key per call, the claim / stage / run loop over a job's groups and the timed gather of the records into `buffer`."""
+
+    _claim_prefix = "pb_claim"              # one per driver class: two drivers of one process group never share a claim counter
+
+    def __init__(self, caller_cls, state: dict, device: int, schedule: str, group_regions: int, distributed: bool, caller):
         import torch
         import torch.distributed as dist
-        from .pipeline import VariantCaller
-        self.world = dist.get_world_size() if dist.is_initialized() else 1
-        self.rank = dist.get_rank() if dist.is_initialized() else 0
-        self.caller = VariantCaller(state, device)
+        on = distributed and dist.is_initialized()
+        self.world = dist.get_world_size() if on else 1
+        self.rank = dist.get_rank() if on else 0
+        self._own_caller = caller is None
+        self.caller = caller if caller is not None else caller_cls(state, device)
         self.device = torch.device("cuda", device)
         self.schedule, self.group_regions = schedule, group_regions
         self.buffer = None
-        self._capacity = capacity
         self._calls = 0
         self._ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
-        self.phase_ms = {}
-        self.groups_done = 0
+        self.phase_ms, self.stats = {}, {}
 
     def close(self):
         """Call before destroy_process_group()."""
         if self.buffer is not None:
             self.buffer.release()
             self.buffer = None
-        self.caller.close()
+        if self._own_caller:
+            self.caller.close()
+
+    def _claimer(self, n_job: int, work: np.ndarray | None) -> GroupClaimer:
+        self._calls += 1
+        return GroupClaimer(n_job, self.rank, self.world, self.schedule, work, key="%s_%d" % (self._claim_prefix, self._calls))
+
+    def _gather_buffer(self, capacity: int, n_job: int, record=PRED_RECORD) -> GatherBuffer:
+        if self.buffer is None or self.buffer.max_groups < n_job or self.buffer.capacity != capacity:
+            if self.buffer is not None:
+                self.buffer.release()
+            self.buffer = GatherBuffer(capacity, self.world, self.rank, self.device, max_groups=n_job, record=record)
+        return self.buffer
+
+    def _run_job(self, s, claimer, groups: list[tuple[int, int]], capacity: int, source=None, stage=None, first=None,
+                 world: int | None = None) -> list[tuple[int, int]]:
+        """run_claimed over the job's groups: group j covers regions groups[j] = [g0, g1) of the source and is staged with region
+        ids from first[j] (default g0).  From a file source (frontend._GroupSource) the fetch of a claimed group starts on the
+        source's fetch ring, one fetch per reader outstanding beside the group being run; otherwise `stage(j)` stages group j."""
+        from .frontend import FETCH_READERS
+        request, depth = None, 1
+        if source is not None:
+            def stage(j):
+                g0, g1 = groups[j]
+                s.stage_device(source.take(j, g0, g1), 0, g1 - g0, g0 if first is None else first[j])
+
+            def request(j):
+                source.request(j, *groups[j])
+            depth = FETCH_READERS
+        return run_claimed(s, claimer, stage, request, depth, capacity, len(groups), world or self.world)
+
+    def _gather(self, s, n: int, segments: list[tuple[int, int]], n_job: int, capacity: str, option: str):
+        """This rank's count and segments into the meta table, both all-gathers (timed: the wait for the slowest rank, then the
+        transfer), then the check that the ranks together ran every group."""
+        import torch
+        t = self.caller.timings()
+        self.stats = s.stats()
+        self.buffer.set_mine(n, segments)
+        self._ev[0].record()
+        self.buffer.gather_meta()                 # tiny: completes when the slowest rank arrives -> the wait, not the transfer
+        self._ev[1].record()
+        self.buffer.gather_records()
+        self._ev[2].record()
+        torch.cuda.synchronize(self.device)
+        self.phase_ms = dict(encoder_ms=t["encode_ms"], network_ms=t["network_ms"], wait_ms=self._ev[0].elapsed_time(self._ev[1]),
+                             gather_ms=self._ev[1].elapsed_time(self._ev[2]), groups=len(segments))
+        check_groups_ran(len(self.buffer.segments()), n_job, capacity, option)
+
+
+class DistributedVariantCaller(_RankDriver):
+    """make_images + run_inference of ONE job (a region list every rank can read) over all ranks of the default process group.
+
+        dvc = DistributedVariantCaller(state, local_device, capacity)
+        dvc.run(source, regions, params)        # source: abi.HostReads (pinned host buffers), pipeline.DeviceReads, or
+                                                # frontend.VariantFileSource (BAM + FASTA every rank opens; regions=None)
+        records = dvc.buffer.to_host()          # every rank holds the whole job's records after the gather
+
+    `capacity`: the records of this rank's slice of the gather buffer; run() fails if the ranks together could not run every
+    group.  `distributed=False` runs the same path on this process alone (world size 1)."""
+
+    def __init__(self, state: dict, device: int, capacity: int, schedule: str = "dynamic", group_regions: int = 32,
+                 distributed: bool = True, caller=None):
+        from .pipeline import VariantCaller
+        super().__init__(VariantCaller, state, device, schedule, group_regions, distributed, caller)
+        self._capacity = capacity
+        self.groups_done = 0
 
     def run(self, source, regions, params: dict, seq_off: np.ndarray | None = None, replicas: int = 1) -> int:
         """Returns this rank's candidate count; the gathered records are in self.buffer (device).
         `replicas` > 1 (benchmarks only): the job is `replicas` copies of the region list laid end to end — job group J is local
         group J mod G with region ids shifted by (J div G) * n_regions — so that a weak-scaling run can hand out N x the
         per-GPU block without holding N copies of it."""
-        import torch
         from .abi import HostReads, regions_array
         from .frontend import VariantFileSource
         from .pipeline import DeviceReads
@@ -370,58 +439,32 @@ class DistributedVariantCaller:
             w_plain, w_last = group_work(seq_off, regions.table, plain), group_work(seq_off, regions.table, last)
             work = np.concatenate([np.tile(w_plain, replicas - 1), w_last])
         n_job = len(job)
-        if self.buffer is None or self.buffer.max_groups < n_job:
-            self.buffer = GatherBuffer(self._capacity, self.world, self.rank, self.device, max_groups=n_job)
-        self._calls += 1
-        claimer = GroupClaimer(n_job, self.rank, self.world, self.schedule, work, key="pb_claim_%d" % self._calls)
-        s = self.caller.stream(params, self.buffer.capacity, d_records=self.buffer.my_ptr())
-        depth = 1                                 # groups claimed ahead of the one being run
-        if from_files:
-            from .frontend import FETCH_READERS
-            depth = FETCH_READERS                 # fetches (pread + H2D + inflate) outstanding beside the group being run: one per reader of
-                                                  # the source's rotation (the reader of the group just taken is free again)
-
+        cap = self._gather_buffer(self._capacity, n_job).capacity
+        claimer = self._claimer(n_job, work)
+        s = self.caller.stream(params, cap, d_records=self.buffer.my_ptr())
+        groups = [(g0, g1) for _, g0, g1 in job]
+        first = [rep * n_reg + g0 for rep, g0, _ in job]
+        stage = None
+        if isinstance(source, DeviceReads):
             def stage(j):
-                rep, g0, g1 = job[j]
-                s.stage_device(source.take(j, g0, g1), 0, g1 - g0, rep * n_reg + g0)
-        elif isinstance(source, DeviceReads):
-            def stage(j):
-                rep, g0, g1 = job[j]
-                s.stage_device(source, g0, g1, rep * n_reg + g0)
-        else:
+                s.stage_device(source, *groups[j], first[j])
+        elif not from_files:
             assert isinstance(source, HostReads)
             regs, keep = regions_array(regions)
             ref = np.ascontiguousarray(regions.ref, dtype=np.uint8)
 
             def stage(j):
-                rep, g0, g1 = job[j]
-                s.stage_host(source, regs, g0, g1, ref, rep * n_reg + g0)
-        request = (lambda j: source.request(j, job[j][1], job[j][2])) if from_files else None
-        segments = run_claimed(s, claimer, stage, request, depth, self.buffer.capacity, n_job, self.world)
+                s.stage_host(source, regs, *groups[j], ref, first[j])
+        segments = self._run_job(s, claimer, groups, cap, source if from_files else None, stage, first)
         n = s.end()
         self.groups_done = len(segments)
-        t = self.caller.timings()
-        self.stats = s.stats()
-        self.buffer.set_mine(n, segments)
-        self._ev[0].record()
-        self.buffer.gather_meta()                 # tiny: completes when the slowest rank arrives -> the wait, not the transfer
-        self._ev[1].record()
-        self.buffer.gather_records()
-        self._ev[2].record()
-        torch.cuda.synchronize(self.device)
-        self.phase_ms = dict(encoder_ms=t["encode_ms"], network_ms=t["network_ms"], wait_ms=self._ev[0].elapsed_time(self._ev[1]),
-                             gather_ms=self._ev[1].elapsed_time(self._ev[2]), groups=len(segments))
-        if self.schedule == "dynamic" and self.world > 1:
-            done = int((self.buffer.meta[:, 1::2] >= 0).sum().item())
-            if done != n_job:
-                raise RuntimeError("only %d of %d groups were run: every rank's record capacity (%d) is exhausted — raise `capacity`"
-                                   % (done, n_job, self.buffer.capacity))
+        self._gather(s, n, segments, n_job, "every rank's record capacity (%d)" % cap, "capacity")
         return n
 
 
-def plan_polish_groups(regions_per_contig: list[int], group: int = 32) -> list[tuple[int, int]]:
-    """Groups [g0, g1) of a polish job whose regions are laid out contig after contig: runs of at most `group` whole regions
-    that never cross a contig, so that each group's consensus belongs to one contig."""
+def plan_contig_groups(regions_per_contig: list[int], group: int = 32) -> list[tuple[int, int]]:
+    """Groups [g0, g1) of a job whose regions are laid out contig after contig: runs of at most `group` whole regions that never
+    cross a contig, so that each group's output belongs to one contig."""
     out, base = [], 0
     for n in regions_per_contig:
         out.extend((base + a, base + b) for a, b in plan_groups(int(n), group))
@@ -429,7 +472,10 @@ def plan_polish_groups(regions_per_contig: list[int], group: int = 32) -> list[t
     return out
 
 
-class DistributedPolisher:
+plan_polish_groups = plan_contig_groups          # the name the polish path first published; callers importing it keep working
+
+
+class DistributedPolisher(_RankDriver):
     """make_images + call_consensus + stitch of ONE assembly (every contig of a frontend.PolishFileSource) over all ranks of the
     default process group.  Each rank runs a streaming polish session (pipeline.PolishStream) over the groups it claims; the
     stitch kernel writes the consensus bases straight into this rank's slice of one byte gather buffer, and a single all-gather
@@ -443,82 +489,33 @@ class DistributedPolisher:
     upper bound of its consensus bytes) leave too little room, and run() fails if the ranks together could not run every
     group.  `distributed=False` runs the same path on this process alone (world size 1)."""
 
+    _claim_prefix = "pb_polish_claim"
+
     def __init__(self, state: dict, device: int, capacity_bytes: int, schedule: str = "dynamic", group_regions: int = 32,
                  distributed: bool = True, caller=None):
-        import torch
-        import torch.distributed as dist
         from .pipeline import PolishCaller
-        on = distributed and dist.is_initialized()
-        self.world = dist.get_world_size() if on else 1
-        self.rank = dist.get_rank() if on else 0
-        self._own_caller = caller is None
-        self.caller = caller if caller is not None else PolishCaller(state, device)
-        self.device = torch.device("cuda", device)
-        self.schedule, self.group_regions = schedule, group_regions
+        super().__init__(PolishCaller, state, device, schedule, group_regions, distributed, caller)
         self.capacity = int(capacity_bytes)
-        self.buffer = None
-        self._calls = 0
-        self._ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
-        self.phase_ms, self.stats = {}, {}
-
-    def close(self):
-        """Call before destroy_process_group()."""
-        if self.buffer is not None:
-            self.buffer.release()
-            self.buffer = None
-        if self._own_caller:
-            self.caller.close()
 
     def run(self, source) -> int:
         """Returns this rank's consensus bytes; the gathered bytes of every rank are in self.buffer (device)."""
-        import torch
-        from .frontend import FETCH_READERS
         groups = source.groups(self.group_regions)
         n_job = len(groups)
-        if self.buffer is None or self.buffer.max_groups < n_job or self.buffer.capacity != self.capacity:
-            if self.buffer is not None:
-                self.buffer.release()
-            self.buffer = GatherBuffer(self.capacity, self.world, self.rank, self.device, max_groups=n_job, record=np.uint8)
-        self._calls += 1
-        claimer = GroupClaimer(n_job, self.rank, self.world, self.schedule, source.group_work(groups), key="pb_polish_claim_%d" % self._calls)
+        self._gather_buffer(self.capacity, n_job, np.uint8)
+        claimer = self._claimer(n_job, source.group_work(groups))
         s = self.caller.stream(self.capacity, self.buffer.my_ptr())
-
-        def stage(j):
-            g0, g1 = groups[j]
-            s.stage_device(source.take(j, g0, g1), 0, g1 - g0, g0)
-
-        def request(j):
-            source.request(j, *groups[j])
-        # one fetch per reader of the source's rotation outstanding beside the group being run
-        segments = run_claimed(s, claimer, stage, request, FETCH_READERS, self.capacity, n_job, self.world)
+        segments = self._run_job(s, claimer, groups, self.capacity, source)
         n = s.end()
-        exact = s.group_bytes()
-        segments = [(g, int(k)) for (g, _), k in zip(segments, exact)]
-        t = self.caller.timings()
-        self.stats = s.stats()
-        self.buffer.set_mine(n, segments)
-        self._ev[0].record()
-        self.buffer.gather_meta()                 # tiny: completes when the slowest rank arrives -> the wait, not the transfer
-        self._ev[1].record()
-        self.buffer.gather_records()
-        self._ev[2].record()
-        torch.cuda.synchronize(self.device)
-        self.phase_ms = dict(encoder_ms=t["encode_ms"], network_ms=t["network_ms"], wait_ms=self._ev[0].elapsed_time(self._ev[1]),
-                             gather_ms=self._ev[1].elapsed_time(self._ev[2]), groups=len(segments))
-        done = int((self.buffer.meta[:, 1::2] >= 0).sum().item())
-        if done != n_job:
-            from ._lib import PepperB200Error
-            from .abi import PB_ERR_CAPACITY
-            raise PepperB200Error("only %d of %d groups were run: the consensus capacity (%d bytes per rank) is exhausted — raise "
-                                  "`capacity_bytes`" % (done, n_job, self.capacity), PB_ERR_CAPACITY)
+        segments = [(g, int(k)) for (g, _), k in zip(segments, s.group_bytes())]
+        self._gather(s, n, segments, n_job, "the consensus capacity (%d bytes per rank)" % self.capacity, "capacity_bytes")
         return n
 
     def assemble(self, source) -> dict:
         """{contig: polished sequence} of every contig of the source's plan (empty string: nothing survived), on every rank:
         the gathered bytes in group order, cut at the contig boundaries of the plan."""
         groups = source.groups(self.group_regions)
-        return assemble_contigs(self.buffer.to_host(), self.buffer.segments(), [source.contig_of_region(g0) for g0, _ in groups],
-                                source.contigs)
+        return assemble_contigs(self.buffer.to_host(), self.buffer.segments(), [source.names[source.contig_of[g0]] for g0, _ in groups],
+                                source.names)
 
 
 def assemble_contigs(data: np.ndarray, segments: list[tuple[int, int]], group_contig: list[str], contigs: list[str]) -> dict:
@@ -645,7 +642,7 @@ def parse_rank_bytes(data) -> dict:
     return out
 
 
-class DistributedGenomeCaller:
+class DistributedGenomeCaller(_RankDriver):
     """`pepper_variant call_variant -b -f -o -s [-r]` of a whole genome over all ranks of the default process group.
 
         dgc = DistributedGenomeCaller(state, local_device, capacity_bytes)
@@ -662,26 +659,14 @@ class DistributedGenomeCaller:
     `capacity_bytes`: the candidate records one rank's session may hold (84 bytes each); run fails when the ranks together could
     not run every group.  `distributed=False` runs alone at world size 1."""
 
+    _claim_prefix = "pb_genome_claim"
+
     def __init__(self, state: dict, device: int, capacity_bytes: int, schedule: str = "dynamic", group_regions: int = 32,
                  distributed: bool = True, caller=None):
-        import torch
-        import torch.distributed as dist
         from .pipeline import VariantCaller
-        on = distributed and dist.is_initialized()
-        self.world = dist.get_world_size() if on else 1
-        self.rank = dist.get_rank() if on else 0
-        self._own_caller = caller is None
-        self.caller = caller if caller is not None else VariantCaller(state, device)
+        super().__init__(VariantCaller, state, device, schedule, group_regions, distributed, caller)
         self.device_id = device
-        self.device = torch.device("cuda", device)
-        self.schedule, self.group_regions = schedule, group_regions
         self.capacity = int(capacity_bytes)
-        self._calls = 0
-        self.phase_ms = {}
-
-    def close(self):
-        if self._own_caller:
-            self.caller.close()
 
     # ---------------------------------------------------------------- per-rank work
     def run_groups(self, src, claimer, params: dict, options: dict | None = None, vcf_options: dict | None = None,
@@ -692,7 +677,6 @@ class DistributedGenomeCaller:
         import torch
         from .abi import PbCandidateColumns, regions_array, ALLELE_STRIDE
         from .candidates import ONT_OPTIONS
-        from .frontend import FETCH_READERS
         from .vcf import vcf_text_device, VCF_LINE
         from ._lib import check
         groups = src.groups(self.group_regions)
@@ -701,14 +685,7 @@ class DistributedGenomeCaller:
         cap = max(1, self.capacity // RECORD_BYTES)
         t0 = time.perf_counter()
         s = self.caller.stream(params, cap)
-
-        def stage(j):
-            g0, g1 = groups[j]
-            s.stage_device(src.take(j, g0, g1), 0, g1 - g0, g0)
-
-        def request(j):
-            src.request(j, *groups[j])
-        segments = run_claimed(s, claimer, stage, request, FETCH_READERS, cap, len(groups), world or self.world)
+        segments = self._run_job(s, claimer, groups, cap, src, world=world)
         n = s.end()
         part.groups = sorted(g for g, _ in segments)
         part.phase_ms["sessions"] = (time.perf_counter() - t0) * 1e3
@@ -886,26 +863,20 @@ class DistributedGenomeCaller:
         from .frontend import VariantGenomeSource
         from .synth import ont_params
         from .vcf import write_vcfs_from_parts
-        from ._lib import PepperB200Error
-        from .abi import PB_ERR_CAPACITY
         params = params or ont_params()
         src = VariantGenomeSource(bam, fasta, int(params["min_snp_baseq"]), region, exclude, interval_size, self.device_id,
                                   gpu_inflate=gpu_inflate)
         try:
             groups = src.groups(self.group_regions)
-            self._calls += 1
-            claimer = GroupClaimer(len(groups), self.rank, self.world, self.schedule, src.group_work(groups),
-                                   key="pb_genome_claim_%d" % self._calls)
-            part = self.run_groups(src, claimer, params, options, vcf_options)
+            part = self.run_groups(src, self._claimer(len(groups), src.group_work(groups)), params, options, vcf_options)
             t0 = time.perf_counter()
             held = self._all_gather_object(part.held)
             held = np.concatenate(held) if held else np.zeros(0, PRED_RECORD)
             part.phase_ms["edge_exchange"] = (time.perf_counter() - t0) * 1e3
             self.edge_pass(part, src, held, options, vcf_options)
             table = sum(self._all_gather_object(group_table_rows(part, len(groups))))
-            if int(table[:, GT_RAN].sum()) != len(groups):
-                raise PepperB200Error("only %d of %d groups were run: the session capacity (%d bytes per rank) is exhausted — raise "
-                                      "`capacity_bytes`" % (int(table[:, GT_RAN].sum()), len(groups), self.capacity), PB_ERR_CAPACITY)
+            check_groups_ran(int(table[:, GT_RAN].sum()), len(groups), "the session capacity (%d bytes per rank)" % self.capacity,
+                             "capacity_bytes")
             totals = self.compress(part, src, table)
             t0 = time.perf_counter()
             got = self._gather_bytes(part)

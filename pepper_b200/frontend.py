@@ -9,6 +9,7 @@ from __future__ import annotations
 
 import ctypes as C
 import re
+import time
 
 import numpy as np
 
@@ -41,6 +42,18 @@ def polish_intervals(interval_start: int, interval_end: int, max_size: int = 100
 def variant_intervals(interval_start: int, interval_end: int, region_size: int = 100_000) -> list[tuple[int, int]]:
     """pepper_variant ImageGenerationUI.py:307-316."""
     return [(max(interval_start, pos), min(interval_end, pos + region_size)) for pos in range(interval_start, interval_end, region_size)]
+
+
+def variant_rows(intervals: list[tuple[int, int]]) -> tuple[list[list[int]], list[tuple[int, int]]]:
+    """Region-table rows of variant intervals and the reference span of each: the interval widened by REGION_SAFE_BASES
+    (AlignmentSummarizer.py:181-182), its reference get_reference_sequence(.., region_end + 1)."""
+    rows = [[max(0, s - REGION_SAFE_BASES), e + REGION_SAFE_BASES, s, e, 0, 0, 0, 0] for s, e in intervals]
+    return rows, [(r[0], r[1] + 1) for r in rows]
+
+
+def polish_rows(regions_se: list[tuple[int, int]]) -> tuple[list[list[int]], list[tuple[int, int]]]:
+    """Region-table rows of polish regions and the reference span of each (AlignmentSummarizer.py:164-170)."""
+    return [[s, e, s, e, 0, 0, 0, 0] for s, e in regions_se], [(s, e + ALIGNMENT_SAFE_BASES) for s, e in regions_se]
 
 
 class _FromFiles:
@@ -96,6 +109,9 @@ class _FromFiles:
     def __exit__(self, *a):
         self.close()
 
+    def fasta_contigs(self) -> list[tuple[str, int]]:
+        return [(c, self.fasta.get_chromosome_sequence_length(c)) for c in self.fasta.get_chromosome_names()]
+
     def _fetch(self, reader, contig: str, beg: int, end: int):
         return reader.fetch_device(contig, beg, end, self.device) if self.gpu_inflate else reader.fetch(contig, beg, end)
 
@@ -114,12 +130,9 @@ class _FromFiles:
                       min_mapq: int = 0, max_reads: int = VARIANT_MAX_READS, downsample_rate: float = 1.0, prof: dict | None = None):
         """Reference strings + batched get_reads of one batch of variant intervals on the side stream (synchronous for the host):
         fetched records -> the FetchedReads the encoder consumes."""
-        import time
         t1 = time.perf_counter()
-        rows, queries, spans = [], [], []
-        for (a, b) in g:
-            rs, re_ = max(0, a - REGION_SAFE_BASES), b + REGION_SAFE_BASES
-            queries.append((rs, re_)); rows.append([rs, re_, a, b, 0, 0, 0, 0]); spans.append((rs, re_ + 1))
+        rows, spans = variant_rows(g)
+        queries = [(r[0], r[1]) for r in rows]
         regions = self._ref_table(contig, rows, spans)
         t2 = time.perf_counter()
         side = self._side_stream()
@@ -141,6 +154,52 @@ class _FromFiles:
         return RegionTable(np.array(rows, dtype=np.int64).reshape(-1, 8), ref if ref.shape[0] else np.zeros(1, np.uint8))
 
 
+class _FetchRing:
+    """BAM fetches of a streaming call on a helper thread: FETCH_WORKERS fetches at once (the pread of one span beside the inflate
+    of another), each on its own reader of `src`, FETCH_READERS readers in rotation, so that the records of the group being
+    trimmed stay valid while later spans are read and inflated.  The caller keeps at most FETCH_READERS requests outstanding
+    and waits for them in request order.  Given `prof`, the helper thread's fetch time is added to prof["fetch_thread"] and the
+    caller's wait to prof["wait_fetch"] (seconds)."""
+
+    def __init__(self, src: _FromFiles, prof: dict | None = None):
+        from concurrent.futures import ThreadPoolExecutor
+        self._src, self._prof = src, prof
+        self._ring = src._readers(FETCH_READERS)
+        self._pool = ThreadPoolExecutor(max_workers=FETCH_WORKERS)
+        self._futs, self._issued = {}, 0
+
+    def request(self, key, contig: str, beg: int, end: int) -> None:
+        reader = self._ring[self._issued % FETCH_READERS]
+        self._issued += 1
+        self._futs[key] = self._pool.submit(self._fetch, reader, contig, beg, end)
+
+    def _fetch(self, reader, contig: str, beg: int, end: int):
+        t0 = time.perf_counter()
+        view = self._src._fetch(reader, contig, beg, end)
+        if self._prof is not None:
+            self._prof["fetch_thread"] += time.perf_counter() - t0
+        return view
+
+    def wait(self, key):
+        """The fetched view of request `key`."""
+        t0 = time.perf_counter()
+        view = self._futs.pop(key).result()            # a Future re-raises the worker's exception (bad contig, corrupt block) here
+        if self._prof is not None:
+            self._prof["wait_fetch"] += time.perf_counter() - t0
+        return view
+
+    def close(self):
+        """Waits for the fetches still in flight, so that their readers are free again."""
+        self._pool.shutdown(wait=True)
+        self._futs = {}
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+
 class VariantFromFiles(_FromFiles):
     """call_variant's make_images + run_inference for a list of intervals of one contig."""
 
@@ -155,14 +214,10 @@ class VariantFromFiles(_FromFiles):
         import torch
         if not intervals:
             raise ValueError("no intervals")
-        rows, queries, spans = [], [], []
-        for (s, e) in intervals:
-            rs, re_ = max(0, s - REGION_SAFE_BASES), e + REGION_SAFE_BASES          # AlignmentSummarizer.py:181-182
-            queries.append((rs, re_))                                               # get_reads(chrom, region_start, region_end, ...)
-            rows.append([rs, re_, s, e, 0, 0, 0, 0])
-            spans.append((rs, re_ + 1))                                             # get_reference_sequence(.., region_end + 1)
+        rows, spans = variant_rows(intervals)
+        queries = [(r[0], r[1]) for r in rows]                                      # get_reads(chrom, region_start, region_end, ...)
         regions = self._ref_table(contig, rows, spans)
-        view = _view if _view is not None else self._fetch(self.bam, contig, min(q[0] for q in queries), max(q[1] for q in queries))
+        view = _view if _view is not None else self._fetch(self.bam, contig, *self._group_span(intervals))
         got = self.trimmer.get_reads(view, queries, include_supplementary, min_mapq, int(params["min_snp_baseq"]),
                                      max_reads=max_reads, downsample_rate=downsample_rate)
         fetched = FetchedReads(got, regions, self.device)
@@ -210,11 +265,8 @@ class VariantFromFiles(_FromFiles):
         readers = self._readers(2)
         groups = [intervals[i:i + batch] for i in range(0, len(intervals), batch)]
 
-        def span(g):
-            return max(0, min(s for s, _ in g) - REGION_SAFE_BASES), max(e for _, e in g) + REGION_SAFE_BASES
-
         def prefetch(k):
-            return self._fetch(readers[k & 1], contig, *span(groups[k]))
+            return self._fetch(readers[k & 1], contig, *self._group_span(groups[k]))
         # a Future re-raises the worker's exception (bad contig, corrupt BGZF block) in the consumer
         with ThreadPoolExecutor(max_workers=1) as pool:
             fut = pool.submit(prefetch, 0)
@@ -233,41 +285,24 @@ class VariantFromFiles(_FromFiles):
         candidates accumulate on the device and the network runs over whole 9,472-candidate chunks across batch boundaries.
         `region_of` counts intervals from the start of the list.  `_finish(session, n)`, when given, replaces the D2H fetch of the
         candidates (they are still in the session's device buffers) and its result is returned."""
-        from concurrent.futures import ThreadPoolExecutor
         if not intervals:
             raise ValueError("no intervals")
-        readers = self._readers(FETCH_READERS)
         groups = [intervals[i:i + batch] for i in range(0, len(intervals), batch)]
-
-        def prefetch(k):
-            return self._fetch(readers[k % FETCH_READERS], contig, *self._group_span(groups[k]))
-        import time
         cap = capacity or max(4096, int(sum(e - s + 1 for s, e in intervals)) // 30)
         prof = dict(wait_fetch=0.0, ref_table=0.0, get_reads=0.0, stage=0.0, run=0.0, sync=0.0, end_fetch=0.0, fetch_thread=0.0)
-
-        def timed_prefetch(k):
-            t0 = time.perf_counter()
-            v = prefetch(k)
-            prof["fetch_thread"] += time.perf_counter() - t0
-            return v
-        def trim(view, g):
-            return self._trim_variant(view, contig, g, int(params["min_snp_baseq"]), include_supplementary, min_mapq, max_reads,
-                                      downsample_rate, prof)
         while True:
             s = self.caller.stream(params, cap)
             try:
-                with ThreadPoolExecutor(max_workers=FETCH_WORKERS) as pool:
-                    # FETCH_WORKERS fetches run at once (the pread of one batch beside the inflate of another), each on its own
-                    # reader; batch j + FETCH_READERS is requested on the reader of batch j as soon as j's records are trimmed
-                    futs = {k: pool.submit(timed_prefetch, k) for k in range(min(FETCH_READERS, len(groups)))}
+                with _FetchRing(self, prof) as ring:
+                    # batch j + FETCH_READERS is requested on the reader of batch j as soon as j's records are trimmed
+                    for k in range(min(FETCH_READERS, len(groups))):
+                        ring.request(k, contig, *self._group_span(groups[k]))
 
                     def take(k):
-                        t0 = time.perf_counter()
-                        view = futs.pop(k).result()
-                        prof["wait_fetch"] += time.perf_counter() - t0
-                        fetched = trim(view, groups[k])
+                        fetched = self._trim_variant(ring.wait(k), contig, groups[k], int(params["min_snp_baseq"]), include_supplementary,
+                                                     min_mapq, max_reads, downsample_rate, prof)
                         if k + FETCH_READERS < len(groups):
-                            futs[k + FETCH_READERS] = pool.submit(timed_prefetch, k + FETCH_READERS)
+                            ring.request(k + FETCH_READERS, contig, *self._group_span(groups[k + FETCH_READERS]))
                         return fetched
                     nxt = take(0)
                     done = 0
@@ -298,17 +333,10 @@ class VariantFromFiles(_FromFiles):
 
     def genome_table(self, contig: str, intervals: list[tuple[int, int]]) -> RegionTable:
         """The region table + reference of a whole interval list, rows as the streaming session's groups build them."""
-        rows, spans = [], []
-        for (a, b) in intervals:
-            rs, re_ = max(0, a - REGION_SAFE_BASES), b + REGION_SAFE_BASES
-            rows.append([rs, re_, a, b, 0, 0, 0, 0]); spans.append((rs, re_ + 1))
-        return self._ref_table(contig, rows, spans)
+        return self._ref_table(contig, *variant_rows(intervals))
 
     def vcf_job(self, region: str | None = None, exclude=()) -> list[tuple[str, int, int]]:
         return variant_job(self.fasta_contigs(), self.bam.get_chromosome_sequence_names(), region, exclude)
-
-    def fasta_contigs(self) -> list[tuple[str, int]]:
-        return [(c, self.fasta.get_chromosome_sequence_length(c)) for c in self.fasta.get_chromosome_names()]
 
     def call_genome(self, out_dir: str, sample_name: str, region: str | None = None, exclude=(), params: dict | None = None,
                     options: dict | None = None, vcf_options: dict | None = None, batch: int = 32, **kw) -> tuple:
@@ -361,48 +389,73 @@ class VariantFromFiles(_FromFiles):
         return totals
 
 
-class VariantFileSource(_FromFiles):
-    """The read source of dist.DistributedVariantCaller for a job given as FILES: every rank opens the same coordinate-sorted BAM
-    (+ .bai) and FASTA and turns the interval groups it claims into trimmed device reads (GPU inflate -> record parse -> batched
-    get_reads), so that make_images + run_inference of one contig shard over the ranks from the alignment file itself — no rank
-    reads, inflates or copies a block outside the groups it runs.  `request(key, g0, g1)` starts the fetch of intervals[g0:g1] on a
-    helper thread (FETCH_WORKERS fetches at once, FETCH_READERS readers in rotation, so the records of the group being trimmed stay
-    valid while later spans are read and inflated — the caller keeps at most FETCH_READERS requests outstanding and takes them in
-    request order); `take(key, g0, g1)` waits for it and returns the FetchedReads of that group."""
+class _GroupSource(_FromFiles):
+    """The read source of the dist drivers: a job every rank opens as the same files (coordinate-sorted BAM + .bai, FASTA), laid
+    out contig after contig — contig `names`, `intervals`, the first interval of each contig (+ the total) and `contig_of`, the
+    contig id of each interval.  Groups (`groups`) are runs of whole intervals that never cross a contig.  A rank turns the
+    groups it claims into trimmed device reads, so no rank reads, inflates or copies a block outside the groups it runs.
+    `request(key, g0, g1)` starts the fetch of group [g0, g1)'s BAM span on the fetch ring (_FetchRing); `take(key, g0, g1)`
+    waits for it and returns the group's FetchedReads.  A subclass sets the plan (`_set_plan`) and gives a group's BAM span
+    (`_span`) and the trim of its fetched records (`_trim`)."""
 
-    def __init__(self, bam_path: str, fasta_path: str, contig: str, intervals: list[tuple[int, int]], min_snp_baseq: int,
-                 device: int = 0, threads: int = 0, gpu_inflate: bool = True, include_supplementary: bool = False, min_mapq: int = 0,
-                 downsample_rate: float = 1.0, max_reads: int = VARIANT_MAX_READS, host_share: float | None = None):
-        from concurrent.futures import ThreadPoolExecutor
+    def __init__(self, bam_path: str, fasta_path: str, device: int, threads: int, gpu_inflate: bool, host_share: float | None):
         super().__init__(bam_path, fasta_path, device, threads, gpu_inflate, host_share)
-        self._ring = self._readers(FETCH_READERS)
-        self.contig, self.intervals = contig, list(intervals)
-        self._filters = (int(min_snp_baseq), include_supplementary, min_mapq, max_reads, downsample_rate)
-        self._pool = ThreadPoolExecutor(max_workers=FETCH_WORKERS)
-        self._futs, self._issued = {}, 0
+        self._ring = _FetchRing(self)
+
+    def _set_plan(self, names: list[str], intervals: list[tuple[int, int]], first: list[int]):
+        self.names, self.intervals, self._first = list(names), list(intervals), list(first)
+        self.contig_of = np.repeat(np.arange(len(self.names), dtype=np.int32), np.diff(self._first))
 
     @property
     def n_regions(self) -> int:
         return len(self.intervals)
 
-    def interval_work(self) -> np.ndarray:
-        """Interval lengths: the work estimate the static schedule balances when the read counts are not known before the fetch."""
-        return np.array([e - s + 1 for s, e in self.intervals], dtype=np.int64)
+    def regions_per_contig(self) -> list[int]:
+        return np.diff(self._first).tolist()
+
+    def groups(self, group_regions: int = 32) -> list[tuple[int, int]]:
+        from .dist import plan_contig_groups
+        return plan_contig_groups(self.regions_per_contig(), group_regions)
 
     def request(self, key, g0: int, g1: int) -> None:
-        reader = self._ring[self._issued % FETCH_READERS]
-        self._issued += 1
-        self._futs[key] = self._pool.submit(self._fetch, reader, self.contig, *self._group_span(self.intervals[g0:g1]))
+        self._ring.request(key, self.names[self.contig_of[g0]], *self._span(self.intervals[g0:g1]))
 
     def take(self, key, g0: int, g1: int) -> FetchedReads:
-        view = self._futs.pop(key).result()            # a Future re-raises the worker's exception (bad contig, corrupt block) here
-        return self._trim_variant(view, self.contig, self.intervals[g0:g1], *self._filters)
+        return self._trim(self._ring.wait(key), self.names[self.contig_of[g0]], self.intervals[g0:g1])
 
     def close(self):
-        if getattr(self, "_pool", None) is not None:
-            self._pool.shutdown(wait=True)
-            self._pool = None
+        if getattr(self, "_ring", None) is not None:
+            self._ring.close()
+            self._ring = None
         super().close()
+
+
+class _VariantSource(_GroupSource):
+    """Groups of variant intervals: a group's BAM span is its intervals widened by REGION_SAFE_BASES, and its records are trimmed
+    by get_reads with the filters of VariantFromFiles.call, on the side stream."""
+
+    def __init__(self, bam_path: str, fasta_path: str, min_snp_baseq: int, device: int, threads: int, gpu_inflate: bool,
+                 include_supplementary: bool, min_mapq: int, downsample_rate: float, max_reads: int, host_share: float | None):
+        super().__init__(bam_path, fasta_path, device, threads, gpu_inflate, host_share)
+        self._filters = (int(min_snp_baseq), include_supplementary, min_mapq, max_reads, downsample_rate)
+
+    def _span(self, intervals: list[tuple[int, int]]) -> tuple[int, int]:
+        return self._group_span(intervals)
+
+    def _trim(self, view, contig: str, intervals: list[tuple[int, int]]) -> FetchedReads:
+        return self._trim_variant(view, contig, intervals, *self._filters)
+
+
+class VariantFileSource(_VariantSource):
+    """The read source of dist.DistributedVariantCaller for a job given as FILES: the given intervals of one contig, so that
+    make_images + run_inference of one contig shard over the ranks from the alignment file itself."""
+
+    def __init__(self, bam_path: str, fasta_path: str, contig: str, intervals: list[tuple[int, int]], min_snp_baseq: int,
+                 device: int = 0, threads: int = 0, gpu_inflate: bool = True, include_supplementary: bool = False, min_mapq: int = 0,
+                 downsample_rate: float = 1.0, max_reads: int = VARIANT_MAX_READS, host_share: float | None = None):
+        super().__init__(bam_path, fasta_path, min_snp_baseq, device, threads, gpu_inflate, include_supplementary, min_mapq,
+                         downsample_rate, max_reads, host_share)
+        self._set_plan([contig], intervals, [0, len(intervals)])
 
 
 def genome_plan(fasta_contigs: list[tuple[str, int]], bam_contigs: list[str], region: str | None = None, exclude=(),
@@ -428,39 +481,18 @@ def group_boundaries(intervals: list[tuple[int, int]], first: list[int], groups:
                      for g0, g1 in groups], np.int64).reshape(-1, 2)
 
 
-class VariantGenomeSource(_FromFiles):
+class VariantGenomeSource(_VariantSource):
     """The read source of dist.DistributedGenomeCaller: every contig of variant_job (the contigs call_genome processes, with the
-    same `region` / `exclude` handling), each tiled with variant_intervals(start, end, interval_size), the intervals laid out
-    contig after contig.  Groups (`groups`) are runs of whole intervals that never cross a contig; `request` / `take` fetch and
-    trim a group's reads as VariantFileSource does.  Contig id k is the k-th contig of the job (call_genome's numbering)."""
+    same `region` / `exclude` handling), each tiled with variant_intervals(start, end, interval_size).  Contig id k is the k-th
+    contig of the job (call_genome's numbering)."""
 
     def __init__(self, bam_path: str, fasta_path: str, min_snp_baseq: int, region: str | None = None, exclude=(),
                  interval_size: int = 100_000, device: int = 0, threads: int = 0, gpu_inflate: bool = True,
                  include_supplementary: bool = False, min_mapq: int = 0, downsample_rate: float = 1.0,
                  max_reads: int = VARIANT_MAX_READS, host_share: float | None = None):
-        from concurrent.futures import ThreadPoolExecutor
-        super().__init__(bam_path, fasta_path, device, threads, gpu_inflate, host_share)
-        self.names, self.intervals, self._first = genome_plan(self.fasta_contigs(), self.bam.get_chromosome_sequence_names(), region,
-                                                             exclude, interval_size)
-        self.contig_of = np.repeat(np.arange(len(self.names), dtype=np.int32), np.diff(self._first))
-        self._filters = (int(min_snp_baseq), include_supplementary, min_mapq, max_reads, downsample_rate)
-        self._ring = self._readers(FETCH_READERS)
-        self._pool = ThreadPoolExecutor(max_workers=FETCH_WORKERS)
-        self._futs, self._issued = {}, 0
-
-    def fasta_contigs(self) -> list[tuple[str, int]]:
-        return [(c, self.fasta.get_chromosome_sequence_length(c)) for c in self.fasta.get_chromosome_names()]
-
-    @property
-    def n_regions(self) -> int:
-        return len(self.intervals)
-
-    def regions_per_contig(self) -> list[int]:
-        return [self._first[k + 1] - self._first[k] for k in range(len(self.names))]
-
-    def groups(self, group_regions: int = 32) -> list[tuple[int, int]]:
-        from .dist import plan_polish_groups
-        return plan_polish_groups(self.regions_per_contig(), group_regions)
+        super().__init__(bam_path, fasta_path, min_snp_baseq, device, threads, gpu_inflate, include_supplementary, min_mapq,
+                         downsample_rate, max_reads, host_share)
+        self._set_plan(*genome_plan(self.fasta_contigs(), self.bam.get_chromosome_sequence_names(), region, exclude, interval_size))
 
     def boundaries(self, groups: list[tuple[int, int]]) -> np.ndarray:
         return group_boundaries(self.intervals, self._first, groups)
@@ -478,31 +510,11 @@ class VariantGenomeSource(_FromFiles):
         for r in sorted(int(x) for x in regions):
             by_contig.setdefault(int(self.contig_of[r]), []).append(r)
         for k, rs in by_contig.items():
-            rr, spans = [], []
-            for r in rs:
-                a, b = self.intervals[r]
-                s, e = max(0, a - REGION_SAFE_BASES), b + REGION_SAFE_BASES
-                rr.append([s, e, a, b, 0, 0, 0, 0]); spans.append((s, e + 1))
-            t = self._ref_table(self.names[k], rr, spans)
+            t = self._ref_table(self.names[k], *variant_rows([self.intervals[r] for r in rs]))
             t.table[:, 4] += base
             rows[rs] = t.table
             refs.append(t.ref); base += t.ref.shape[0]
         return RegionTable(rows, np.concatenate(refs) if refs else np.zeros(1, np.uint8))
-
-    def request(self, key, g0: int, g1: int) -> None:
-        reader = self._ring[self._issued % FETCH_READERS]
-        self._issued += 1
-        self._futs[key] = self._pool.submit(self._fetch, reader, self.names[self.contig_of[g0]], *self._group_span(self.intervals[g0:g1]))
-
-    def take(self, key, g0: int, g1: int) -> FetchedReads:
-        view = self._futs.pop(key).result()            # a Future re-raises the worker's exception (bad contig, corrupt block) here
-        return self._trim_variant(view, self.names[self.contig_of[g0]], self.intervals[g0:g1], *self._filters)
-
-    def close(self):
-        if getattr(self, "_pool", None) is not None:
-            self._pool.shutdown(wait=True)
-            self._pool = None
-        super().close()
 
 
 class PolishFromFiles(_FromFiles):
@@ -519,11 +531,7 @@ class PolishFromFiles(_FromFiles):
         import torch
         if not regions_se:
             raise ValueError("no regions")
-        rows, spans = [], []
-        for (rs, re_) in regions_se:
-            rows.append([rs, re_, rs, re_, 0, 0, 0, 0])
-            spans.append((rs, re_ + ALIGNMENT_SAFE_BASES))                         # AlignmentSummarizer.py:164-170
-        regions = self._ref_table(contig, rows, spans)
+        regions = self._ref_table(contig, *polish_rows(regions_se))
         view = self._fetch(self.bam, contig, min(r[0] for r in regions_se), max(r[1] for r in regions_se))
         got = self.trimmer.get_reads(view, regions_se, False, 0, 0, max_reads=max_reads, downsample_rate=1.0)   # :300-325
         fetched = FetchedReads(got, regions, self.device)
@@ -545,27 +553,51 @@ class PolishFromFiles(_FromFiles):
         h = {k: v[:n].cpu().numpy() for k, v in out.items()}
         return PolishCalls(h["bases"], h["phred"], h["position"], h["index"], h["image_region"], h["chunk_id"]), fetched_table(fetched, regions)
 
+    def polish_contig(self, contig: str, start: int = 0, end: int | None = None, batch: int = 2000, realign: bool = True,
+                      return_calls: bool = False):
+        """The whole polish path of one contig span: tiling (ImageGenerationUI.py:262-272: the span is [start, length - 1]),
+        make_images + call_consensus in batches of `batch` regions, then the stitch (Stitch.py:36-128) -> polished sequence."""
+        from .polish import stitch
+        if end is None:
+            end = self.fasta.get_chromosome_sequence_length(contig) - 1
+        regs = polish_intervals(start, end)
+        parts = []
+        for i in range(0, len(regs), batch):
+            calls, _ = self.call(contig, regs[i:i + batch], realign=realign)
+            parts.append((calls, i))
+        cat = lambda f: np.concatenate([getattr(c, f) for c, _ in parts])       # noqa: E731
+        image_region = np.concatenate([c.image_region + off for c, off in parts]).astype(np.int32)
+        allc = PolishCalls(cat("bases"), cat("phred"), cat("position"), cat("index"), image_region, cat("chunk_id"))
+        seq = stitch(allc.bases, allc.position, allc.index, allc.image_region, allc.chunk_id, np.array([r[0] for r in regs], dtype=np.int64))
+        return (seq, allc, regs) if return_calls else seq
 
-def _polish_contig(self, contig: str, start: int = 0, end: int | None = None, batch: int = 2000, realign: bool = True,
-                   return_calls: bool = False):
-    """The whole polish path of one contig span: tiling (ImageGenerationUI.py:262-272: the span is [start, length - 1]),
-    make_images + call_consensus in batches of `batch` regions, then the stitch (Stitch.py:36-128) -> polished sequence."""
-    from .polish import stitch
-    if end is None:
-        end = self.fasta.get_chromosome_sequence_length(contig) - 1
-    regs = polish_intervals(start, end)
-    parts = []
-    for i in range(0, len(regs), batch):
-        calls, _ = self.call(contig, regs[i:i + batch], realign=realign)
-        parts.append((calls, i))
-    cat = lambda f: np.concatenate([getattr(c, f) for c, _ in parts])       # noqa: E731
-    image_region = np.concatenate([c.image_region + off for c, off in parts]).astype(np.int32)
-    allc = PolishCalls(cat("bases"), cat("phred"), cat("position"), cat("index"), image_region, cat("chunk_id"))
-    seq = stitch(allc.bases, allc.position, allc.index, allc.image_region, allc.chunk_id, np.array([r[0] for r in regs], dtype=np.int64))
-    return (seq, allc, regs) if return_calls else seq
-
-
-PolishFromFiles.polish_contig = _polish_contig
+    def polish_assembly(self, out_path: str | None = None, contigs: list[str] | None = None, group_regions: int = 32,
+                        capacity_bytes: int | None = None, realign: bool = True) -> dict:
+        """`pepper polish` of a whole assembly on this GPU: every contig common to the BAM and the FASTA (or `contigs`),
+        make_images + call_consensus + the stitch on the device through one streaming session (dist.DistributedPolisher at world
+        size 1).  Returns {contig: polished sequence} and, given `out_path`, writes the FASTA perform_stitch writes."""
+        from .dist import DistributedPolisher
+        src = PolishFileSource(self.bam.path, self.fasta_path, contigs, self.device, self.threads, self.gpu_inflate, realign,
+                               host_share=self.host_share)
+        try:
+            cap = capacity_bytes or 2 * sum(e - s + 1 for s, e in src.intervals) + (1 << 20)
+            while True:
+                dp = DistributedPolisher(None, self.device, cap, "static", group_regions, distributed=False, caller=self.caller)
+                try:
+                    dp.run(src)
+                    seqs = dp.assemble(src)
+                    break
+                except PepperB200Error as ex:        # consensus larger than the sink: restart the session larger
+                    if ex.rc != PB_ERR_CAPACITY:
+                        raise
+                    cap *= 2
+                finally:
+                    dp.close()
+        finally:
+            src.close()
+        if out_path is not None:
+            write_polished_fasta(out_path, seqs)
+        return seqs
 
 
 def natural_key(string_: str) -> list:
@@ -646,58 +678,34 @@ def variant_job(fasta_contigs: list[tuple[str, int]], bam_contigs: list[str], re
     return job
 
 
-class PolishFileSource(_FromFiles):
-    """The read source of dist.DistributedPolisher: a whole assembly given as FILES every rank opens (coordinate-sorted BAM + .bai,
-    FASTA).  The job is every contig common to both files in natural order (ImageGenerationUI.get_chromosome_list, pepper
-    ImageGenerationUI.py:88-117) or the given `contigs`, each tiled with polish_intervals(0, length - 1); regions are numbered
-    contig after contig, and groups (`groups`) are runs of whole regions that never cross a contig.  `request(key, g0, g1)` starts
-    the fetch of a group's BAM span on a helper thread (FETCH_READERS readers in rotation, as VariantFileSource);
-    `take(key, g0, g1)` waits for it and runs get_reads with the filters of PolishFromFiles.call and the realignment on a side
-    stream, so that a group's inflate, trim and realignment run beside the previous group's network."""
+class PolishFileSource(_GroupSource):
+    """The read source of dist.DistributedPolisher: a whole assembly, every contig common to both files in natural order
+    (ImageGenerationUI.get_chromosome_list, pepper ImageGenerationUI.py:88-117) or the given `contigs`, each tiled with
+    polish_intervals(0, length - 1).  `take` runs get_reads with the filters of PolishFromFiles.call and the realignment on a
+    side stream, so that a group's inflate, trim and realignment run beside the previous group's network."""
 
     def __init__(self, bam_path: str, fasta_path: str, contigs: list[str] | None = None, device: int = 0, threads: int = 0,
                  gpu_inflate: bool = True, realign: bool = True, max_reads: int = POLISH_MAX_READS, host_share: float | None = None):
-        from concurrent.futures import ThreadPoolExecutor
         super().__init__(bam_path, fasta_path, device, threads, gpu_inflate, host_share)
-        fasta = [(c, self.fasta.get_chromosome_sequence_length(c)) for c in self.fasta.get_chromosome_names()]
-        self.contigs, self.regions, self._first = polish_job(fasta, self.bam.get_chromosome_sequence_names(), contigs)
-        self._contig_of = [k for k in range(len(self.contigs)) for _ in range(self._first[k + 1] - self._first[k])]
+        self._set_plan(*polish_job(self.fasta_contigs(), self.bam.get_chromosome_sequence_names(), contigs))
         self.realign = realign
         self.realigner = Realigner(device) if realign else None
         self._max_reads = max_reads
-        self._ring = self._readers(FETCH_READERS)
-        self._pool = ThreadPoolExecutor(max_workers=FETCH_WORKERS)
-        self._futs, self._issued = {}, 0
 
     @property
-    def n_regions(self) -> int:
-        return len(self.regions)
-
-    def regions_per_contig(self) -> list[int]:
-        return [self._first[k + 1] - self._first[k] for k in range(len(self.contigs))]
-
-    def contig_of_region(self, r: int) -> str:
-        return self.contigs[self._contig_of[r]]
-
-    def groups(self, group_regions: int = 32) -> list[tuple[int, int]]:
-        from .dist import plan_polish_groups
-        return plan_polish_groups(self.regions_per_contig(), group_regions)
+    def contigs(self) -> list[str]:
+        """The contigs of the assembly, in the order polished (the plan's `names`)."""
+        return self.names
 
     def group_work(self, groups: list[tuple[int, int]]) -> np.ndarray:
         """Draft bases per group: the work estimate the static schedule balances."""
-        return np.array([sum(e - s + 1 for s, e in self.regions[g0:g1]) for g0, g1 in groups], dtype=np.int64)
+        return np.array([sum(e - s + 1 for s, e in self.intervals[g0:g1]) for g0, g1 in groups], dtype=np.int64)
 
-    def request(self, key, g0: int, g1: int) -> None:
-        reader = self._ring[self._issued % FETCH_READERS]
-        self._issued += 1
-        regs = self.regions[g0:g1]
-        self._futs[key] = self._pool.submit(self._fetch, reader, self.contig_of_region(g0), min(s for s, _ in regs), max(e for _, e in regs))
+    def _span(self, regs: list[tuple[int, int]]) -> tuple[int, int]:
+        return min(s for s, _ in regs), max(e for _, e in regs)
 
-    def take(self, key, g0: int, g1: int) -> FetchedReads:
-        view = self._futs.pop(key).result()            # a Future re-raises the worker's exception (bad contig, corrupt block) here
-        contig, regs = self.contig_of_region(g0), self.regions[g0:g1]
-        rows = [[rs, re_, rs, re_, 0, 0, 0, 0] for rs, re_ in regs]
-        regions = self._ref_table(contig, rows, [(rs, re_ + ALIGNMENT_SAFE_BASES) for rs, re_ in regs])     # AlignmentSummarizer.py:164-170
+    def _trim(self, view, contig: str, regs: list[tuple[int, int]]) -> FetchedReads:
+        regions = self._ref_table(contig, *polish_rows(regs))
         side = self._side_stream()
         got = self.trimmer.get_reads(view, regs, False, 0, 0, max_reads=self._max_reads, downsample_rate=1.0, stream=side.cuda_stream)
         fetched = FetchedReads(got, regions, self.device, stream=side)
@@ -706,45 +714,10 @@ class PolishFileSource(_FromFiles):
         return fetched
 
     def close(self):
-        if getattr(self, "_pool", None) is not None:
-            self._pool.shutdown(wait=True)
-            self._pool = None
+        super().close()
         if getattr(self, "realigner", None) is not None:
             self.realigner.close()
             self.realigner = None
-        super().close()
-
-
-def _polish_assembly(self, out_path: str | None = None, contigs: list[str] | None = None, group_regions: int = 32,
-                     capacity_bytes: int | None = None, realign: bool = True) -> dict:
-    """`pepper polish` of a whole assembly on this GPU: every contig common to the BAM and the FASTA (or `contigs`), make_images +
-    call_consensus + the stitch on the device through one streaming session (dist.DistributedPolisher at world size 1).
-    Returns {contig: polished sequence} and, given `out_path`, writes the FASTA perform_stitch writes."""
-    from .dist import DistributedPolisher
-    src = PolishFileSource(self.bam.path, self.fasta_path, contigs, self.device, self.threads, self.gpu_inflate, realign,
-                           host_share=self.host_share)
-    try:
-        cap = capacity_bytes or 2 * sum(e - s + 1 for s, e in src.regions) + (1 << 20)
-        while True:
-            dp = DistributedPolisher(None, self.device, cap, "static", group_regions, distributed=False, caller=self.caller)
-            try:
-                dp.run(src)
-                seqs = dp.assemble(src)
-                break
-            except PepperB200Error as ex:        # consensus larger than the sink: restart the session larger
-                if ex.rc != PB_ERR_CAPACITY:
-                    raise
-                cap *= 2
-            finally:
-                dp.close()
-    finally:
-        src.close()
-    if out_path is not None:
-        write_polished_fasta(out_path, seqs)
-    return seqs
-
-
-PolishFromFiles.polish_assembly = _polish_assembly
 
 
 def fetched_table(fetched: FetchedReads, regions: RegionTable) -> RegionTable:

@@ -54,6 +54,31 @@ def test_static_claimer_blocks():
     assert got[0] + got[1] == list(range(6)) and got[0] and got[1]
 
 
+def test_capacity_stop_is_an_error_under_any_schedule():
+    """run_claimed stops claiming when this rank's slice could not hold another group, under the static schedule and at world
+    size 1 too; the meta table then lists fewer groups than the job has, and that is a capacity error, not a short result."""
+    import pytest
+    from pepper_b200._lib import PepperB200Error
+    from pepper_b200.abi import PB_ERR_CAPACITY
+    from pepper_b200.dist import check_groups_ran, run_claimed
+
+    class Session:                                       # 100 records per group
+        total = 0
+
+        def run(self, flush=False):
+            self.total += 100
+            return self.total
+    segments = run_claimed(Session(), GroupClaimer(10, 0, 1, "static"), lambda j: None, None, 1, 500, 10, 1)
+    assert segments == [(0, 100), (1, 100), (2, 100), (3, 100)]
+    buf = GatherBuffer(500, 1, 0, max_groups=10)
+    buf.gather(400, segments)
+    assert buf.segments() == segments
+    with pytest.raises(PepperB200Error, match="groups were run") as ei:
+        check_groups_ran(len(buf.segments()), 10, "the record capacity (500)", "capacity")
+    assert ei.value.rc == PB_ERR_CAPACITY
+    check_groups_ran(10, 10, "the record capacity (500)", "capacity")
+
+
 def test_order_and_records_from_calls():
     class Calls:
         pass

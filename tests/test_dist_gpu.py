@@ -70,6 +70,30 @@ def test_stream_session_matches_one_shot_call():
     caller.close()
 
 
+def test_distributed_caller_raises_when_capacity_stops_the_claims():
+    """World size 1, static schedule, a record capacity of about a third of the job: the rank stops claiming after a few groups
+    (each fits its session), and run() raises PB_ERR_CAPACITY instead of returning the records of only the first groups."""
+    from oracle import nets
+    from pepper_b200._lib import PepperB200Error
+    from pepper_b200.abi import PB_ERR_CAPACITY
+    from pepper_b200.dist import DistributedVariantCaller, plan_groups
+    from pepper_b200.pipeline import VariantCaller, DeviceReads
+    reads, regions = _workload()
+    params = synth.ont_params()
+    state = nets.make_variant_weights(5)
+    caller = VariantCaller(state)
+    n_job = len(caller.call(reads, regions, params))
+    caller.close()
+    dvc = DistributedVariantCaller(state, 0, capacity=n_job // 3, schedule="static", group_regions=5)
+    try:
+        with pytest.raises(PepperB200Error, match="groups were run") as ei:
+            dvc.run(DeviceReads(reads, regions), regions, params)
+        assert ei.value.rc == PB_ERR_CAPACITY
+        assert 0 < dvc.phase_ms["groups"] < len(plan_groups(regions.n_regions, 5))
+    finally:
+        dvc.close()
+
+
 def _rank_main(rank, world, port, q, paths=None):
     import torch
     import torch.distributed as dist

@@ -52,7 +52,7 @@ def test_vectorised_index_matches_bai_bytes(seed):
 
 
 def test_group_plan_and_boundaries():
-    from pepper_b200.dist import plan_polish_groups
+    from pepper_b200.dist import plan_contig_groups
     from pepper_b200.frontend import genome_plan, group_boundaries
     fasta = [("chr2", 2501), ("chr10", 901), ("chr1", 4201), ("chrM", 1801), ("chr3", 1000)]      # chr3: in the FASTA only
     names, iv, first = genome_plan(fasta, ["chr2", "chr10", "chr1", "chrM"], exclude=("chrM",), interval_size=1000)
@@ -60,17 +60,17 @@ def test_group_plan_and_boundaries():
     per = [first[k + 1] - first[k] for k in range(len(names))]
     assert per == [5, 3, 1]                                   # many intervals, several, one
     assert iv[:5] == [(0, 1000), (1000, 2000), (2000, 3000), (3000, 4000), (4000, 4200)]
-    groups = plan_polish_groups(per, 2)
+    groups = plan_contig_groups(per, 2)
     assert groups == [(0, 2), (2, 4), (4, 5), (5, 7), (7, 8), (8, 9)]
     contig = np.repeat(np.arange(3), per)
     assert all(len(set(contig[g0:g1].tolist())) == 1 for g0, g1 in groups)
     bnd = group_boundaries(iv, first, groups)
     assert bnd.tolist() == [[-1, 2000], [2000, 4000], [4000, -1], [-1, 2000], [2000, -1], [-1, -1]]
-    one = group_boundaries(iv, first, plan_polish_groups(per, 1))
+    one = group_boundaries(iv, first, plan_contig_groups(per, 1))
     assert one[5:8].tolist() == [[-1, 1000], [1000, 2000], [2000, -1]]
     names2, iv2, first2 = genome_plan(fasta, ["chr2", "chr10", "chr1", "chrM"], region="chr2:500-1700,chr10", interval_size=1000)
     assert names2 == ["chr2", "chr10"] and iv2[:2] == [(500, 1500), (1500, 1700)]
-    assert group_boundaries(iv2, first2, plan_polish_groups([2, 1], 1)).tolist() == [[-1, 1500], [1500, -1], [-1, -1]]
+    assert group_boundaries(iv2, first2, plan_contig_groups([2, 1], 1)).tolist() == [[-1, 1500], [1500, -1], [-1, -1]]
 
 
 def _lines(rng, names, n_per):

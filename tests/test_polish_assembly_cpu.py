@@ -9,7 +9,7 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 from oracle import stitch as ostitch
-from pepper_b200.dist import GatherBuffer, GroupClaimer, assemble_contigs, plan_polish_groups
+from pepper_b200.dist import GatherBuffer, GroupClaimer, assemble_contigs, plan_contig_groups
 from pepper_b200.frontend import natural_key, polish_intervals, polish_job, polished_fasta_text
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -39,13 +39,13 @@ def test_natural_order_and_job_plan():
 
 def test_groups_never_cross_contigs():
     per_contig = [3, 1, 0, 70, 5]
-    groups = plan_polish_groups(per_contig, 32)
+    groups = plan_contig_groups(per_contig, 32)
     bounds = np.cumsum([0] + per_contig)
     assert groups[0][0] == 0 and groups[-1][1] == bounds[-1] and all(a[1] == b[0] for a, b in zip(groups, groups[1:]))
     for g0, g1 in groups:
         k = int(np.searchsorted(bounds, g0, side="right")) - 1
         assert bounds[k] <= g0 < g1 <= bounds[k + 1] and g1 - g0 <= 32
-    assert plan_polish_groups(per_contig, 1) == [(r, r + 1) for r in range(bounds[-1])]
+    assert plan_contig_groups(per_contig, 1) == [(r, r + 1) for r in range(bounds[-1])]
 
 
 def _oracle_group_bytes(z, regions):
@@ -90,7 +90,7 @@ def _worker(rank, world, port, q):
     z = _golden()
     contigs = [str(c) for c in z["contigs"]]
     per_contig = [int((z["region_contig"] == k).sum()) for k in range(len(contigs))]
-    groups = plan_polish_groups(per_contig, 1)
+    groups = plan_contig_groups(per_contig, 1)
     group_contig = [contigs[int(z["region_contig"][g0])] for g0, _ in groups]
     buf = GatherBuffer(40000, world, rank, max_groups=len(groups), record=np.uint8)
     c = GroupClaimer(len(groups), rank, world, "dynamic", key="polish")
