@@ -200,7 +200,8 @@ int pb_test_realign_pairs(pb_realigner_t *t, const uint8_t *h_query, const int64
  * faidx_fetch_seq, fasta_handler.cpp:7-50).
  * ---------------------------------------------------------------------- */
 typedef struct pb_bam pb_bam_t;
-/* BAM_handler(path): opens path and path + ".bai" (or name.bai); n_threads <= 0 = all cores (BGZF inflate pool) */
+/* BAM_handler(path): opens path and its index, the first that exists of path.csi, name.csi, path.bai, name.bai (name = path
+ * without ".bam"); n_threads <= 0 = all cores (BGZF inflate pool) */
 int pb_bam_open(pb_bam_t **out, const char *path, int n_threads);
 int pb_bam_close(pb_bam_t *b);
 int pb_bam_n_contigs(pb_bam_t *b);                              /* get_chromosome_sequence_names (bam_handler.cpp:103) */
@@ -212,15 +213,22 @@ const char *pb_bam_header_text(pb_bam_t *b, int64_t *len);     /* get_sample_nam
  * reader-owned host memory (page-locked when a GPU is present; valid until the next fetch / close)                   */
 int pb_bam_fetch(pb_bam_t *b, int tid, int64_t beg, int64_t end, pb_records_t *h_view);
 int pb_bam_io_stats(pb_bam_t *b, int64_t *compressed_bytes, int64_t *inflated_bytes);
+/* the index's reach: both fetches clamp `end` to it, as htslib does; 2^29 for a BAI, 2^(min_shift + 3 depth) for a CSI */
+int64_t pb_bam_index_max_end(pb_bam_t *b);
+/* *is_csi = 1 for a CSI index, 0 for a BAI; its min_shift and depth ((14, 5) for a BAI) */
+int pb_bam_index_info(pb_bam_t *b, int *is_csi, int *min_shift, int *depth);
 
 /* GPU fetch (VERDICT r1 item 5): the same records as pb_bam_fetch, but only the COMPRESSED BGZF blocks are copied to the
- * device; DEFLATE inflate (one warp per BGZF block), the record-chain walk (one thread per BAI linear-index window start), the
+ * device; DEFLATE inflate (one warp per BGZF block), the record-chain walk (one thread per known record start: chunk begins plus
+ * the BAI linear-index entries of the windows, or the CSI loffsets of the bins, the query touches), the
  * record parse and the scatter into the structure-of-arrays are kernels.  `view` receives DEVICE pointers owned by the
  * reader (valid until its next pb_bam_fetch_device) — the input of pb_get_reads_plan_device.  Replaces bgzf_read / bam_read1 /
  * sam_itr_next under BAM_handler::get_reads (bam_handler.cpp:115-135).                                                        */
 int pb_bam_fetch_device(pb_bam_t *bam, int tid, int64_t beg, int64_t end, int device, pb_records_t *view, void *stream);
 /* device time (ms) of the last pb_bam_fetch_device: [H2D + inflate, record chains + parse, scatter] */
 int pb_bam_fetch_device_timings(pb_bam_t *bam, float *ms3);
+/* known record starts of the last pb_bam_fetch_device (one walking thread each) and the most records one thread walked */
+int pb_bam_fetch_device_anchors(pb_bam_t *bam, int64_t *anchors, int64_t *longest_walk);
 /* Hybrid inflate of pb_bam_fetch_device: `share` (0..1) of the BGZF blocks — runs of 16 consecutive blocks — is inflated by the
  * reader's host thread pool (zlib) WHILE the kernel inflates the rest; the host runs reach the same device buffer through a copy
  * stream, and the record kernels wait for both.  Default 0 (everything on the GPU); the environment variable
@@ -237,7 +245,8 @@ int pb_test_inflate_blocks(const uint8_t *h_comp, int64_t comp_bytes, const int6
                            const int32_t *h_out_len, int64_t n_blocks, uint8_t *h_out, int32_t *h_status, void *stream, int spec);
 
 typedef struct pb_fasta pb_fasta_t;
-int pb_fasta_open(pb_fasta_t **out, const char *path);          /* FASTA_handler(path): path + ".fai" must exist       */
+/* FASTA_handler(path): path + ".fai" must exist; a bgzip-compressed FASTA also needs path + ".gzi" (plain gzip is refused) */
+int pb_fasta_open(pb_fasta_t **out, const char *path);
 int pb_fasta_close(pb_fasta_t *f);
 int pb_fasta_n_contigs(pb_fasta_t *f);                          /* get_chromosome_names (fasta_handler.cpp:19)         */
 const char *pb_fasta_contig_name(pb_fasta_t *f, int i);

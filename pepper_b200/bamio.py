@@ -1,5 +1,5 @@
 """File readers under BAM_handler / FASTA_handler (SURVEY.md §8f row f4): ctypes front-end of the host-side BGZF / BAM /
-BAI and FASTA / FAI readers in libpepper_b200.so (pepper_b200/csrc/bamio.cu).  Reference: BAM_handler(path) and its
+BAI / CSI and FASTA / FAI (plain or bgzip + GZI) readers in libpepper_b200.so (pepper_b200/csrc/bamio.cu).  Reference: BAM_handler(path) and its
 accessors (pepper/modules/src/dataio/bam_handler.cpp:6-113), FASTA_handler (fasta_handler.cpp:7-55)."""
 from __future__ import annotations
 
@@ -26,6 +26,10 @@ def _bind(L):
     L.pb_bam_header_text.restype = C.c_void_p
     L.pb_bam_fetch.argtypes = [C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.POINTER(PbRecords)]
     L.pb_bam_io_stats.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+    L.pb_bam_index_max_end.argtypes = [C.c_void_p]
+    L.pb_bam_index_max_end.restype = C.c_int64
+    L.pb_bam_index_info.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    L.pb_bam_fetch_device_anchors.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.pb_bam_fetch_device.argtypes = [C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_int, C.POINTER(PbRecords), C.c_void_p]
     L.pb_bam_fetch_device_timings.argtypes = [C.c_void_p, C.c_void_p]
     L.pb_bam_set_host_share.argtypes = [C.c_void_p, C.c_double]
@@ -152,6 +156,17 @@ class BamReader:
         except Exception:      # noqa: BLE001
             pass
 
+    @property
+    def index_max_end(self) -> int:
+        """The index's reach: no fetch returns a record at or past it (2^29 for a BAI, 2^(min_shift + 3 depth) for a CSI)."""
+        return int(self.L.pb_bam_index_max_end(self.h))
+
+    def index_info(self) -> dict:
+        """{"format": "csi" or "bai", "min_shift", "depth"} of the index the reader opened."""
+        c, m, d = C.c_int(0), C.c_int(0), C.c_int(0)
+        _lib.check(self.L.pb_bam_index_info(self.h, C.byref(c), C.byref(m), C.byref(d)), "pb_bam_index_info")
+        return dict(format="csi" if c.value else "bai", min_shift=int(m.value), depth=int(d.value))
+
     def get_chromosome_sequence_names(self) -> list[str]:                      # bam_handler.cpp:103-113
         return [self.L.pb_bam_contig_name(self.h, i).decode() for i in range(self.L.pb_bam_n_contigs(self.h))]
 
@@ -191,6 +206,13 @@ class BamReader:
         view = PbRecords()
         _lib.check(self.L.pb_bam_fetch_device(self.h, tid, beg, end, device, C.byref(view), C.c_void_p(stream)), "pb_bam_fetch_device")
         return DeviceRecordsView(view, self, device)
+
+    def fetch_device_anchors(self) -> tuple[int, int]:
+        """(known record starts, most records walked from one of them) of the last fetch_device: the walk runs one GPU thread per
+        start, so the second number bounds the walk's length."""
+        a, w = C.c_int64(0), C.c_int64(0)
+        self.L.pb_bam_fetch_device_anchors(self.h, C.byref(a), C.byref(w))
+        return int(a.value), int(w.value)
 
     def fetch_device_timings(self) -> dict:
         ms = (C.c_float * 3)()

@@ -163,17 +163,26 @@ struct HostBuf {                 // grow-only; page-locked when a CUDA device is
 };
 
 struct Chunk { uint64_t beg, end; };
-struct RefIndex { std::map<uint32_t, std::vector<Chunk>> bins; std::vector<uint64_t> linear; };
+// loffset: a CSI bin's lower bound on the virtual offset of any record overlapping the bin (0 in a BAI, which has a linear index)
+struct Bin { uint64_t loffset = 0; std::vector<Chunk> chunks; };
+struct RefIndex { std::map<uint32_t, Bin> bins; std::vector<uint64_t> linear; };
 
-// bins overlapping [beg, end) (SAMv1 5.3 reg2bins)
-void reg2bins(int64_t beg, int64_t end, std::vector<uint32_t> &out) {
+// The binning scheme of a BAI (min_shift 14, depth 5) or a CSI (SAMv1 5.3): level l (0 = the root) has 8^l bins of 2^shift(l)
+// positions, numbered from ((1 << 3l) - 1) / 7.  An index covers [0, 1 << (min_shift + 3 depth)).
+struct Binning {
+    int min_shift = 14, depth = 5;
+    int shift(int l) const { return min_shift + 3 * (depth - l); }
+    static uint32_t first(int l) { return (uint32_t) (((1ull << (3 * l)) - 1) / 7); }
+    int64_t max_end() const { return 1ll << (min_shift + 3 * depth); }
+};
+
+// bins overlapping [beg, end), end <= max_end (SAMv1 5.3 reg2bins)
+void reg2bins(const Binning &bn, int64_t beg, int64_t end, std::vector<uint32_t> &out) {
     --end;
-    out.push_back(0);
-    for (int64_t k = 1 + (beg >> 26); k <= 1 + (end >> 26); ++k) out.push_back((uint32_t) k);
-    for (int64_t k = 9 + (beg >> 23); k <= 9 + (end >> 23); ++k) out.push_back((uint32_t) k);
-    for (int64_t k = 73 + (beg >> 20); k <= 73 + (end >> 20); ++k) out.push_back((uint32_t) k);
-    for (int64_t k = 585 + (beg >> 17); k <= 585 + (end >> 17); ++k) out.push_back((uint32_t) k);
-    for (int64_t k = 4681 + (beg >> 14); k <= 4681 + (end >> 14); ++k) out.push_back((uint32_t) k);
+    for (int l = 0; l <= bn.depth; l++) {
+        const int s = bn.shift(l);
+        for (int64_t k = beg >> s; k <= end >> s; ++k) out.push_back(Binning::first(l) + (uint32_t) k);
+    }
 }
 
 struct RecRef { size_t off; uint32_t l_seq, n_cigar; const uint8_t *cigar; };   // off: start of the record body in the inflated buffer
@@ -189,6 +198,9 @@ struct pb_bam {
     std::vector<std::string> names;
     std::vector<int64_t> lens;
     std::vector<RefIndex> index;
+    Binning binning;                    // (14, 5) for a BAI; a CSI's own
+    bool csi = false;
+    int64_t last_anchors = 0, last_longest_walk = 0;   // of the last pb_bam_fetch_device
     size_t first_record_voff_block = 0;
     // fetch scratch / outputs
     struct RawBuf {                     // grow-only, never zero-filled; contents preserved up to `keep` bytes on growth
@@ -247,6 +259,14 @@ struct pb_fasta {
     struct Entry { std::string name; int64_t len, off, linebases, linewidth; };
     std::vector<Entry> entries;
     std::map<std::string, int> by_name;
+    // bgzip-compressed FASTA: the .fai offsets are uncompressed; gzi[k] = (compressed, uncompressed) offset of BGZF block k,
+    // block 0 = (0, 0) included.  A fetch inflates only the blocks it needs, into its own buffer (no shared state), so fetches on
+    // one handle may run from several threads; the pool is taken with try_lock and a fetch that finds it busy inflates inline.
+    bool bgzf = false;
+    std::vector<std::pair<uint64_t, uint64_t>> gzi;
+    Pool *pool = nullptr;
+    std::mutex pool_mu;
+    ~pb_fasta() { delete pool; }
 };
 
 namespace {
@@ -349,7 +369,7 @@ int load_bai(pb_bam *b, const char *path) {
                 const uint32_t bin = rd32(p + o), n_chunk = rd32(p + o + 4);
                 o += 8;
                 if (o + 16ull * n_chunk > n) goto bad;
-                auto &v = b->index[r].bins[bin];
+                auto &v = b->index[r].bins[bin].chunks;
                 for (uint32_t c = 0; c < n_chunk; c++, o += 16) v.push_back({rd64(p + o), rd64(p + o + 8)});
             }
             if (o + 4 > n) goto bad;
@@ -365,6 +385,117 @@ bad:
     f.close();
     set_error("truncated BAI index %s", path);
     return PB_ERR_ARG;
+}
+
+// CSI (the CSIv1 specification): a BGZF file whose payload is magic "CSI\1", min_shift, depth, l_aux, aux, n_ref, then per
+// reference n_bin and per bin (bin u32, loffset u64, n_chunk, chunks), optionally n_no_coor u64.  No linear index.
+int load_csi(pb_bam *b, const char *path) {
+    MappedFile f;
+    if (!f.open(path)) { set_error("cannot open BAM index %s", path); return PB_ERR_ARG; }
+    std::vector<uint8_t> u;
+    for (size_t off = 0; off < f.n;) {
+        size_t data_off;
+        const size_t bs = bgzf_block_size(f.p, f.n, off, &data_off);
+        if (!bs || bs < data_off + 8) { f.close(); set_error("%s is not a BGZF-compressed CSI index (bad block at offset %zu)", path, off); return PB_ERR_ARG; }
+        const uint32_t isize = rd32(f.p + off + bs - 4);
+        if (isize > 65536) { f.close(); set_error("CSI index %s: block at offset %zu claims %u bytes", path, off, isize); return PB_ERR_ARG; }
+        const size_t at = u.size();
+        u.resize(at + isize);
+        if (isize && !inflate_block(f.p + off + data_off, bs - data_off - 8, u.data() + at, isize)) { f.close(); set_error("CSI index %s: inflate failed", path); return PB_ERR_ARG; }
+        off += bs;
+    }
+    f.close();
+    const uint8_t *p = u.data();
+    const size_t n = u.size();
+    if (n < 16 || memcmp(p, "CSI\1", 4)) { set_error("%s is not a CSI index", path); return PB_ERR_ARG; }
+    const int32_t min_shift = rdi32(p + 4), depth = rdi32(p + 8), l_aux = rdi32(p + 12);
+    // positions are int32 in a BAM record: a reach past 2^32 would only overflow the bin arithmetic
+    if (min_shift < 0 || depth < 0 || min_shift + 3 * depth > 32 || depth > 9) { set_error("CSI index %s: unsupported min_shift %d / depth %d", path, min_shift, depth); return PB_ERR_ARG; }
+    if (l_aux < 0 || 16ull + (uint64_t) l_aux + 4 > n) { set_error("truncated CSI index %s", path); return PB_ERR_ARG; }
+    size_t o = 16 + (size_t) l_aux;
+    const int32_t n_ref = rdi32(p + o); o += 4;
+    if (n_ref < 0) { set_error("CSI index %s: negative n_ref", path); return PB_ERR_ARG; }
+    b->binning.min_shift = min_shift; b->binning.depth = depth;
+    b->index.assign((size_t) n_ref, RefIndex());
+    for (int32_t r = 0; r < n_ref; r++) {
+        if (o + 4 > n) goto bad;
+        {
+            const int32_t n_bin = rdi32(p + o); o += 4;
+            if (n_bin < 0) goto bad;
+            for (int32_t i = 0; i < n_bin; i++) {
+                if (o + 16 > n) goto bad;
+                const uint32_t bin = rd32(p + o);
+                const uint64_t loffset = rd64(p + o + 4);
+                const int32_t n_chunk = rdi32(p + o + 12);
+                o += 16;
+                if (n_chunk < 0 || o + 16ull * (uint64_t) n_chunk > n) goto bad;
+                Bin &v = b->index[r].bins[bin];
+                v.loffset = loffset;
+                for (int32_t c = 0; c < n_chunk; c++, o += 16) v.chunks.push_back({rd64(p + o), rd64(p + o + 8)});
+            }
+        }
+    }
+    if (o != n && o + 8 != n) goto bad;                          // nothing but the optional n_no_coor may follow
+    b->csi = true;
+    return PB_OK;
+bad:
+    set_error("truncated CSI index %s", path);
+    return PB_ERR_ARG;
+}
+
+// The index of `path`, the first that exists of <bam>.csi, <name>.csi, <bam>.bai, <name>.bai (name = path without ".bam").
+// We believe this is htslib's order (CSI first, each extension appended and then substituted); htslib is not available here to
+// confirm it.  A file with both indexes gives the same records through either.
+int load_index(pb_bam *b, const char *path) {
+    const std::string full(path);
+    std::vector<std::string> stems{full};
+    if (full.size() > 4 && full.substr(full.size() - 4) == ".bam") stems.push_back(full.substr(0, full.size() - 4));
+    struct stat st;
+    for (const char *ext : {".csi", ".bai"})
+        for (const std::string &s : stems)
+            if (stat((s + ext).c_str(), &st) == 0) return ext[1] == 'c' ? load_csi(b, (s + ext).c_str()) : load_bai(b, (s + ext).c_str());
+    set_error("cannot open BAM index %s.bai or %s.csi (the BAM file must be indexed)", path, path);
+    return PB_ERR_ARG;
+}
+
+// The chunks of (tid, [beg, end)) from the bin index, sorted and merged (SAMv1 5.1.1), and the virtual offsets known to start a
+// record inside them (`anchors`, optional): the one place pb_bam_fetch and pb_bam_fetch_device turn a query into file spans.
+// Chunks ending at or before min_off are dropped: for a BAI min_off is the linear index at beg's 16 kb window; for a CSI it is the
+// loffset of the deepest bin on the path from beg's leaf bin up to the root that the index holds (hts_itr_query).  Either is only
+// a shortcut: the same records come back without it.  Anchors: the linear index of every window the query touches (BAI) or the
+// loffset of every bin it touches (CSI); the device walk starts a thread at each.
+void select_chunks(const pb_bam *b, const RefIndex &ri, int64_t beg, int64_t end, std::vector<Chunk> &merged, std::vector<uint64_t> *anchors) {
+    const Binning &bn = b->binning;
+    std::vector<uint32_t> bins;
+    reg2bins(bn, beg, end, bins);
+    uint64_t min_off = 0;
+    if (!ri.linear.empty()) {
+        const size_t w = (size_t) (beg >> 14);
+        min_off = ri.linear[std::min(w, ri.linear.size() - 1)];
+        if (w >= ri.linear.size()) min_off = ri.linear.back();
+    } else if (b->csi) {
+        for (int l = bn.depth; l >= 0; l--) {
+            auto it = ri.bins.find(Binning::first(l) + (uint32_t) (beg >> bn.shift(l)));
+            if (it != ri.bins.end()) { min_off = it->second.loffset; break; }
+        }
+    }
+    std::vector<Chunk> chunks;
+    for (uint32_t bin : bins) {
+        auto it = ri.bins.find(bin);
+        if (it == ri.bins.end()) continue;
+        for (const Chunk &c : it->second.chunks) if (c.end > min_off) chunks.push_back(c);
+        if (anchors && b->csi) anchors->push_back(it->second.loffset);
+    }
+    std::sort(chunks.begin(), chunks.end(), [](const Chunk &a, const Chunk &c) { return a.beg < c.beg; });
+    merged.clear();
+    for (const Chunk &c : chunks) {
+        if (!merged.empty() && c.beg <= merged.back().end) merged.back().end = std::max(merged.back().end, c.end);
+        else merged.push_back(c);
+    }
+    if (anchors && !ri.linear.empty()) {
+        const size_t w0 = (size_t) (beg >> 14), w1 = std::min((size_t) ((end - 1) >> 14), ri.linear.size() - 1);
+        for (size_t w = w0; w <= w1 && w < ri.linear.size(); w++) anchors->push_back(ri.linear[w]);
+    }
 }
 
 }  // namespace
@@ -384,16 +515,7 @@ extern "C" int pb_bam_open(pb_bam_t **out, const char *path, int n_threads) {
     b->pinned = cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0;
     if (!b->pinned) cudaGetLastError();
     int rc = load_header(b);
-    if (rc == PB_OK) {
-        std::string bai = std::string(path) + ".bai";
-        struct stat st;
-        if (stat(bai.c_str(), &st) != 0) {                       // also accept name.bai next to name.bam
-            std::string alt(path);
-            if (alt.size() > 4 && alt.substr(alt.size() - 4) == ".bam") alt = alt.substr(0, alt.size() - 4) + ".bai";
-            if (stat(alt.c_str(), &st) == 0) bai = alt;
-        }
-        rc = load_bai(b, bai.c_str());
-    }
+    if (rc == PB_OK) rc = load_index(b, path);
     if (rc != PB_OK) { b->f.close(); delete b->pool; delete b; return rc; }
     *out = b;
     return PB_OK;
@@ -436,13 +558,30 @@ extern "C" int pb_bam_io_stats(pb_bam_t *b, int64_t *compressed, int64_t *inflat
     if (inflated) *inflated = b->n_inflated;
     return PB_OK;
 }
+// the index's reach: a fetch sees no record at or past it (2^29 for a BAI, 2^(min_shift + 3 depth) for a CSI); -1 on a null handle
+extern "C" int64_t pb_bam_index_max_end(pb_bam_t *b) { return b ? b->binning.max_end() : -1; }
+// the index format (1 = CSI, 0 = BAI) and its binning
+extern "C" int pb_bam_index_info(pb_bam_t *b, int *is_csi, int *min_shift, int *depth) {
+    if (!b) return PB_ERR_ARG;
+    if (is_csi) *is_csi = b->csi ? 1 : 0;
+    if (min_shift) *min_shift = b->binning.min_shift;
+    if (depth) *depth = b->binning.depth;
+    return PB_OK;
+}
+// record-start anchors of the last pb_bam_fetch_device (one walking thread each) and the most records one of them walked
+extern "C" int pb_bam_fetch_device_anchors(pb_bam_t *b, int64_t *anchors, int64_t *longest_walk) {
+    if (!b) return PB_ERR_ARG;
+    if (anchors) *anchors = b->last_anchors;
+    if (longest_walk) *longest_walk = b->last_longest_walk;
+    return PB_OK;
+}
 
 extern "C" int pb_bam_fetch(pb_bam_t *b, int tid, int64_t beg, int64_t end, pb_records_t *view) {
     if (!b || !view) { set_error("null argument"); return PB_ERR_ARG; }
     memset(view, 0, sizeof(*view));
     if (tid < 0 || tid >= (int) b->names.size()) { set_error("contig id %d out of range", tid); return PB_ERR_ARG; }
     if (beg < 0) beg = 0;
-    if (end > (1ll << 29)) end = 1ll << 29;
+    if (end > b->binning.max_end()) end = b->binning.max_end();            // the index's reach, as htslib clamps (2^29 for a BAI)
     static const bool dbg = getenv("PB_BAM_DEBUG") != nullptr;
     auto tnow = []() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
     const double t_start = tnow();
@@ -452,27 +591,8 @@ extern "C" int pb_bam_fetch(pb_bam_t *b, int tid, int64_t beg, int64_t end, pb_r
     std::vector<int64_t> rpos;
     std::vector<Block> blocks;
     if (end > beg && tid < (int) b->index.size()) {
-        const RefIndex &ri = b->index[tid];
-        std::vector<uint32_t> bins;
-        reg2bins(beg, end, bins);
-        uint64_t min_off = 0;
-        if (!ri.linear.empty()) {
-            const size_t w = (size_t) (beg >> 14);
-            min_off = ri.linear[std::min(w, ri.linear.size() - 1)];
-            if (w >= ri.linear.size()) min_off = ri.linear.back();
-        }
-        std::vector<Chunk> chunks;
-        for (uint32_t bin : bins) {
-            auto it = ri.bins.find(bin);
-            if (it == ri.bins.end()) continue;
-            for (const Chunk &c : it->second) if (c.end > min_off) chunks.push_back(c);
-        }
-        std::sort(chunks.begin(), chunks.end(), [](const Chunk &a, const Chunk &c) { return a.beg < c.beg; });
         std::vector<Chunk> merged;
-        for (const Chunk &c : chunks) {
-            if (!merged.empty() && c.beg <= merged.back().end) merged.back().end = std::max(merged.back().end, c.end);
-            else merged.push_back(c);
-        }
+        select_chunks(b, b->index[tid], beg, end, merged, nullptr);
         if (!merged.empty()) {
             // one inflate pass over the whole span of the merged chunks would decompress gaps too; inflate per chunk group:
             // chunks whose block ranges touch are handled together
@@ -635,35 +755,6 @@ extern "C" int pb_bam_fetch(pb_bam_t *b, int tid, int64_t beg, int64_t end, pb_r
 }
 
 
-namespace {
-
-// chunks of (tid, [beg, end)) from the bin index, clipped by the linear index, sorted and merged (SAMv1 5.1.1) — the same selection
-// pb_bam_fetch makes
-void select_chunks(const RefIndex &ri, int64_t beg, int64_t end, std::vector<Chunk> &merged) {
-    std::vector<uint32_t> bins;
-    reg2bins(beg, end, bins);
-    uint64_t min_off = 0;
-    if (!ri.linear.empty()) {
-        const size_t w = (size_t) (beg >> 14);
-        min_off = ri.linear[std::min(w, ri.linear.size() - 1)];
-        if (w >= ri.linear.size()) min_off = ri.linear.back();
-    }
-    std::vector<Chunk> chunks;
-    for (uint32_t bin : bins) {
-        auto it = ri.bins.find(bin);
-        if (it == ri.bins.end()) continue;
-        for (const Chunk &c : it->second) if (c.end > min_off) chunks.push_back(c);
-    }
-    std::sort(chunks.begin(), chunks.end(), [](const Chunk &a, const Chunk &c) { return a.beg < c.beg; });
-    merged.clear();
-    for (const Chunk &c : chunks) {
-        if (!merged.empty() && c.beg <= merged.back().end) merged.back().end = std::max(merged.back().end, c.end);
-        else merged.push_back(c);
-    }
-}
-
-}  // namespace
-
 // GPU fetch: same records as pb_bam_fetch (file order, htslib overlap rule), delivered as a pb_records_t whose pointers are DEVICE
 // pointers owned by the reader (valid until its next pb_bam_fetch_device), ready for pb_get_reads_plan_device.
 extern "C" int pb_bam_fetch_device(pb_bam_t *b, int tid, int64_t beg, int64_t end, int device, pb_records_t *view, void *stream_) {
@@ -679,9 +770,11 @@ extern "C" int pb_bam_fetch_device(pb_bam_t *b, int tid, int64_t beg, int64_t en
     cudaStream_t st = stream_ ? (cudaStream_t) stream_ : b->own_stream;
     for (auto &e : b->dev_evt) if (!e) PB_CUDA(cudaEventCreate(&e));
     if (beg < 0) beg = 0;
-    if (end > (1ll << 29)) end = 1ll << 29;
+    if (end > b->binning.max_end()) end = b->binning.max_end();
+    b->last_anchors = b->last_longest_walk = 0;
     std::vector<Chunk> merged;
-    if (end > beg && tid < (int) b->index.size()) select_chunks(b->index[tid], beg, end, merged);
+    std::vector<uint64_t> anchors;
+    if (end > beg && tid < (int) b->index.size()) select_chunks(b, b->index[tid], beg, end, merged, &anchors);
     // ---- block list of every chunk group (groups = chunks whose block ranges touch), compressed bytes into one pinned buffer
     struct Group { size_t c0, c1_end; size_t first_block, n_blocks; uint64_t vbeg, vend; size_t chunk0, chunk1; };
     std::vector<Group> groups;
@@ -738,7 +831,8 @@ extern "C" int pb_bam_fetch_device(pb_bam_t *b, int tid, int64_t beg, int64_t en
             if (got != (ssize_t) S.len) memcpy(cb + S.dst_off, b->f.p + S.file_off, S.len);
         });
     }
-    // ---- known record starts: chunk begins + the linear-index entries of the windows the query touches
+    // ---- known record starts: chunk begins + the anchors of select_chunks (linear-index entries of the windows the query touches
+    //      for a BAI, loffsets of the bins it touches for a CSI)
     auto upos = [&](uint64_t voff) -> int64_t {
         const size_t coff = (size_t) (voff >> 16);
         auto it = std::lower_bound(blocks.begin(), blocks.end(), coff, [](const Block &k, size_t c) { return k.coff < c; });
@@ -747,21 +841,16 @@ extern "C" int pb_bam_fetch_device(pb_bam_t *b, int tid, int64_t beg, int64_t en
         return (int64_t) (it->uoff + (size_t) (voff & 0xffff));
     };
     std::vector<int64_t> starts, stops;
-    const RefIndex &ri = b->index[tid];
     for (const Group &G : groups) {
         const Block &lastb = blocks[G.first_block + G.n_blocks - 1];
         int64_t limit = upos(G.vend);
         if (limit < 0) limit = (int64_t) (lastb.uoff + lastb.isize);              // chunk end beyond the last needed block
         std::vector<int64_t> s;
         for (size_t ci = G.chunk0; ci <= G.chunk1; ci++) { const int64_t u0 = upos(merged[ci].beg); if (u0 >= 0 && u0 < limit) s.push_back(u0); }
-        if (!ri.linear.empty()) {
-            const size_t w0 = (size_t) (beg >> 14), w1 = std::min((size_t) ((end - 1) >> 14), ri.linear.size() - 1);
-            for (size_t w = w0; w <= w1 && w < ri.linear.size(); w++) {
-                const uint64_t v = ri.linear[w];
-                if (v < G.vbeg || v >= G.vend) continue;
-                const int64_t u0 = upos(v);
-                if (u0 >= 0 && u0 < limit) s.push_back(u0);
-            }
+        for (const uint64_t v : anchors) {
+            if (v < G.vbeg || v >= G.vend) continue;
+            const int64_t u0 = upos(v);
+            if (u0 >= 0 && u0 < limit) s.push_back(u0);
         }
         std::sort(s.begin(), s.end());
         s.erase(std::unique(s.begin(), s.end()), s.end());
@@ -835,10 +924,14 @@ extern "C" int pb_bam_fetch_device(pb_bam_t *b, int tid, int64_t beg, int64_t en
         k_scan_excl<<<1, 1024, 0, st>>>(b->d_counts.as<int32_t>(), b->d_base.as<int64_t>(), n_starts, sc + 0);
     }
     std::vector<int> h_status((size_t) n_dev + 1);
+    std::vector<int32_t> h_counts((size_t) n_starts + 1, 0);      // records walked from each anchor (reported, not used)
     int64_t h_sc[5] = {0, 0, 0, 0, 0};
     if (n_dev > 0) PB_CUDA(cudaMemcpyAsync(h_status.data(), b->d_status.p, sizeof(int) * n_dev, cudaMemcpyDeviceToHost, st));
+    if (n_starts > 0) PB_CUDA(cudaMemcpyAsync(h_counts.data(), b->d_counts.p, sizeof(int32_t) * n_starts, cudaMemcpyDeviceToHost, st));
     PB_CUDA(cudaMemcpyAsync(h_sc, sc, sizeof(h_sc), cudaMemcpyDeviceToHost, st));
     PB_CUDA(cudaStreamSynchronize(st));
+    b->last_anchors = n_starts;
+    b->last_longest_walk = n_starts > 0 ? *std::max_element(h_counts.begin(), h_counts.begin() + n_starts) : 0;
     for (int64_t i = 0; i < n_dev; i++)
         if (h_status[i]) { set_error("BGZF inflate failed on the GPU: block at file offset %zu, status %d", blocks[dev_block[i]].coff, h_status[i]); return PB_ERR_ARG; }
     if ((int) h_sc[4]) { set_error("BAM record chain is inconsistent with the index (code %d)", (int) h_sc[4]); return PB_ERR_ARG; }
@@ -964,6 +1057,24 @@ extern "C" int pb_fasta_open(pb_fasta_t **out, const char *path) {
     if (!out || !path) { set_error("null argument"); return PB_ERR_ARG; }
     auto *f = new pb_fasta();
     if (!f->f.open(path)) { delete f; set_error("cannot open FASTA file %s", path); return PB_ERR_ARG; }
+    if (f->f.n >= 2 && f->f.p[0] == 0x1f && f->f.p[1] == 0x8b) {
+        size_t d;
+        if (!bgzf_block_size(f->f.p, f->f.n, 0, &d)) { f->f.close(); delete f; set_error("%s is compressed with gzip, not bgzip: it cannot be indexed for random access", path); return PB_ERR_ARG; }
+        const std::string gzi = std::string(path) + ".gzi";
+        MappedFile g;
+        if (!g.open(gzi.c_str())) { f->f.close(); delete f; set_error("cannot open %s: a bgzip-compressed FASTA needs its .gzi index", gzi.c_str()); return PB_ERR_ARG; }
+        const uint64_t n_entries = g.n >= 8 ? rd64(g.p) : 0;
+        if (g.n < 8 || g.n != 8 + 16 * n_entries) { g.close(); f->f.close(); delete f; set_error("malformed .gzi index %s", gzi.c_str()); return PB_ERR_ARG; }
+        f->gzi.emplace_back(0, 0);
+        for (uint64_t i = 0; i < n_entries; i++) f->gzi.emplace_back(rd64(g.p + 8 + 16 * i), rd64(g.p + 16 + 16 * i));
+        g.close();
+        for (size_t i = 1; i < f->gzi.size(); i++)
+            if (f->gzi[i].first <= f->gzi[i - 1].first || f->gzi[i].second < f->gzi[i - 1].second || f->gzi[i].first >= f->f.n) {
+                f->f.close(); delete f; set_error("malformed .gzi index %s: offsets out of order or past the file", gzi.c_str()); return PB_ERR_ARG;
+            }
+        f->bgzf = true;
+        f->pool = new Pool(std::min(8, usable_cores()) - 1);
+    }
     MappedFile idx;
     const std::string fai = std::string(path) + ".fai";
     if (!idx.open(fai.c_str())) { f->f.close(); delete f; set_error("cannot open FASTA index %s (file must be indexed)", fai.c_str()); return PB_ERR_ARG; }
@@ -1019,13 +1130,50 @@ extern "C" int pb_fasta_fetch(pb_fasta_t *f, const char *name, int64_t start, in
     *len = n;
     if (n > cap) return PB_ERR_CAPACITY;
     if (!out || n <= 0) return PB_OK;
+    // the bytes of [b, en] in the file's line layout are [u0, u1): straight from the mapping, or from the BGZF blocks that hold them
+    auto byte_of = [&](int64_t i) { return e.off + (i / e.linebases) * e.linewidth + i % e.linebases; };
+    const int64_t u0 = byte_of(b), u1 = byte_of(en) + 1;
+    const uint8_t *src = f->f.p;
+    size_t src_n = f->f.n;
+    int64_t base = 0;
+    std::vector<uint8_t> ubuf;
+    if (f->bgzf) {
+        auto block_of = [&](int64_t u) {
+            return (size_t) (std::upper_bound(f->gzi.begin(), f->gzi.end(), (uint64_t) u, [](uint64_t v, const std::pair<uint64_t, uint64_t> &g) { return v < g.second; }) - f->gzi.begin()) - 1;
+        };
+        const size_t k0 = block_of(u0), k1 = block_of(u1 - 1);
+        std::vector<Block> blocks;
+        size_t total = 0;
+        for (size_t k = k0; k <= k1; k++) {
+            size_t data_off;
+            const size_t coff = (size_t) f->gzi[k].first;
+            const size_t bs = bgzf_block_size(f->f.p, f->f.n, coff, &data_off);
+            if (!bs || bs < data_off + 8) { set_error("corrupt BGZF block at offset %zu of the FASTA", coff); return PB_ERR_ARG; }
+            const uint32_t isize = rd32(f->f.p + coff + bs - 4);
+            const bool next_ok = k + 1 < f->gzi.size() ? (f->gzi[k + 1].first == coff + bs && f->gzi[k + 1].second == f->gzi[k].second + isize) : true;
+            if (isize > 65536 || !next_ok) { set_error("the .gzi index does not match the BGZF blocks of the FASTA at offset %zu", coff); return PB_ERR_ARG; }
+            blocks.push_back({coff, data_off, bs, isize, total});
+            total += isize;
+        }
+        ubuf.resize(total + 1);
+        std::atomic<int> bad(0);
+        auto one = [&](size_t i) {
+            const Block &k = blocks[i];
+            if (k.isize && !inflate_block(f->f.p + k.coff + k.data_off, k.bsize - k.data_off - 8, ubuf.data() + k.uoff, k.isize)) bad = 1;
+        };
+        std::unique_lock<std::mutex> lk(f->pool_mu, std::try_to_lock);
+        if (lk.owns_lock()) f->pool->run(blocks.size(), one);
+        else for (size_t i = 0; i < blocks.size(); i++) one(i);
+        if (bad) { set_error("BGZF inflate failed in the FASTA"); return PB_ERR_ARG; }
+        src = ubuf.data(); src_n = total; base = (int64_t) f->gzi[k0].second;
+    }
     int64_t w = 0;
     for (int64_t i = b; i <= en;) {
-        const int64_t line = i / e.linebases, col = i % e.linebases;
+        const int64_t col = i % e.linebases;
         const int64_t take = std::min(e.linebases - col, en - i + 1);
-        const int64_t off = e.off + line * e.linewidth + col;
-        if ((size_t) (off + take) > f->f.n) { set_error("FASTA index points past the end of the file"); return PB_ERR_ARG; }
-        memcpy(out + w, f->f.p + off, (size_t) take);
+        const int64_t off = byte_of(i) - base;
+        if (off < 0 || (size_t) (off + take) > src_n) { set_error("FASTA index points past the end of the file"); return PB_ERR_ARG; }
+        memcpy(out + w, src + off, (size_t) take);
         w += take; i += take;
     }
     return PB_OK;

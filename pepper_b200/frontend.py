@@ -336,7 +336,7 @@ class VariantFromFiles(_FromFiles):
         return self._ref_table(contig, *variant_rows(intervals))
 
     def vcf_job(self, region: str | None = None, exclude=()) -> list[tuple[str, int, int]]:
-        return variant_job(self.fasta_contigs(), self.bam.get_chromosome_sequence_names(), region, exclude)
+        return variant_job(self.fasta_contigs(), self.bam.get_chromosome_sequence_names(), region, exclude, self.bam.index_max_end)
 
     def call_genome(self, out_dir: str, sample_name: str, region: str | None = None, exclude=(), params: dict | None = None,
                     options: dict | None = None, vcf_options: dict | None = None, batch: int = 32, **kw) -> tuple:
@@ -355,13 +355,16 @@ class VariantFromFiles(_FromFiles):
         names = [c for c, _, _ in job]
         params = params or ont_params()
         parts = []
-        prof = dict(calls=0.0, vcf=0.0, write=0.0, encoder_device=0.0, network_device=0.0)
+        prof = dict(calls=0.0, vcf=0.0, write=0.0, encoder_device=0.0, network_device=0.0, bam_fetch=0.0, fasta_fetch=0.0)
+        n_groups = 0
         dev = torch.device("cuda", self.device)
         for cid, (contig, start, end) in enumerate(job):
             intervals = variant_intervals(start, end)
             if not intervals:
                 continue
+            t0 = time.perf_counter()
             table = self.genome_table(contig, intervals)
+            prof["fasta_fetch"] += time.perf_counter() - t0
 
             def finish(s, n, table=table, cid=cid):
                 dev_ms = self.caller.timings()                              # the session's encoder / network device time
@@ -378,14 +381,19 @@ class VariantFromFiles(_FromFiles):
             t0 = time.perf_counter()
             parts.append(self.call_stream(contig, intervals, params, batch, _finish=finish, **kw))
             prof["calls"] += time.perf_counter() - t0
+            # the helper thread's BAM fetches and the groups' reference fetches (inside ref_table) of this contig's session
+            prof["bam_fetch"] += self.last_profile["fetch_thread"] / 1e3; prof["fasta_fetch"] += self.last_profile["ref_table"] / 1e3
+            n_groups += -(-len(intervals) // batch)
         t0 = time.perf_counter()
         text, lines = order_lines(parts, names)
         totals = write_vcfs(out_dir, sample_name, self.fasta_contigs(), names, text, lines)
         prof["write"] = time.perf_counter() - t0
         prof["calls"] -= prof["vcf"]
         # ms per stage of the last call: host wall of the sessions, of the VCF pass (synchronous) and of the writer; device time
-        # of the encoder and the network
+        # of the encoder and the network; host time of the BAM fetches (helper thread) and of the FASTA fetches (the whole-contig
+        # tables and each group's reference); "groups" is the number of groups (not a time)
         self.last_genome_profile = {k: round(v * 1e3, 2) for k, v in prof.items()}
+        self.last_genome_profile["groups"] = n_groups
         return totals
 
 
@@ -459,10 +467,11 @@ class VariantFileSource(_VariantSource):
 
 
 def genome_plan(fasta_contigs: list[tuple[str, int]], bam_contigs: list[str], region: str | None = None, exclude=(),
-                interval_size: int = 100_000):
+                interval_size: int = 100_000, max_end: int | None = None):
     """The job of a whole-genome call: the contigs of variant_job, each tiled with variant_intervals(start, end, interval_size),
-    the intervals laid out contig after contig.  Returns (contig names, intervals, first interval of each contig + the total)."""
-    job = variant_job(fasta_contigs, bam_contigs, region, exclude)
+    the intervals laid out contig after contig.  Returns (contig names, intervals, first interval of each contig + the total).
+    `max_end`: the BAM index's reach (variant_job)."""
+    job = variant_job(fasta_contigs, bam_contigs, region, exclude, max_end)
     intervals, first = [], []
     for _, s, e in job:
         first.append(len(intervals))
@@ -492,7 +501,8 @@ class VariantGenomeSource(_VariantSource):
                  max_reads: int = VARIANT_MAX_READS, host_share: float | None = None):
         super().__init__(bam_path, fasta_path, min_snp_baseq, device, threads, gpu_inflate, include_supplementary, min_mapq,
                          downsample_rate, max_reads, host_share)
-        self._set_plan(*genome_plan(self.fasta_contigs(), self.bam.get_chromosome_sequence_names(), region, exclude, interval_size))
+        self._set_plan(*genome_plan(self.fasta_contigs(), self.bam.get_chromosome_sequence_names(), region, exclude, interval_size,
+                                    self.bam.index_max_end))
 
     def boundaries(self, groups: list[tuple[int, int]]) -> np.ndarray:
         return group_boundaries(self.intervals, self._first, groups)
@@ -617,14 +627,16 @@ def polished_fasta_text(seqs: dict) -> str:
     return "".join(">%s\n%s\n" % (c, seqs[c]) for c in sorted(seqs, key=natural_key) if seqs[c])
 
 
-def polish_job(fasta_contigs: list[tuple[str, int]], bam_contigs: list[str], contigs: list[str] | None = None):
+def polish_job(fasta_contigs: list[tuple[str, int]], bam_contigs: list[str], contigs: list[str] | None = None,
+               max_end: int | None = None):
     """The job of a whole-assembly polish: every contig common to the FASTA (name, length) and the BAM, in natural order
     (ImageGenerationUI.get_chromosome_list, pepper ImageGenerationUI.py:88-117), or `contigs`; each contig tiled with
     polish_intervals(0, length - 1) (a contig too short to tile has no region).  Returns (contigs, regions laid out contig after
-    contig, first region of each contig + the total)."""
+    contig, first region of each contig + the total).  `max_end`: the BAM index's reach; a longer contig raises ValueError."""
     lengths = dict(fasta_contigs)
     if contigs is None:
         contigs = sorted(set(lengths) & set(bam_contigs), key=natural_key)
+    check_reach([(c, lengths[c]) for c in contigs if c in lengths], max_end)
     regions, first = [], []
     for c in contigs:
         first.append(len(regions))
@@ -658,23 +670,37 @@ def parse_region(region: str) -> list[tuple[str, tuple[int, int] | None]]:
     return out
 
 
-def variant_job(fasta_contigs: list[tuple[str, int]], bam_contigs: list[str], region: str | None = None, exclude=()):
+def check_reach(spans: list[tuple[str, int]], max_end: int | None) -> None:
+    """Raise ValueError when a contig would be processed up to an end (exclusive) past `max_end`, the BAM index's reach: a fetch
+    returns no read at or past it (a BAI addresses positions below 2^29), so that part of the contig would get no reads."""
+    if max_end is None:
+        return
+    for c, end in spans:
+        if end > max_end:
+            raise ValueError("contig %r is processed up to position %d, but the BAM index only addresses positions below %d: "
+                             "index the BAM with a CSI of enough depth (samtools index -c)" % (c, end, max_end))
+
+
+def variant_job(fasta_contigs: list[tuple[str, int]], bam_contigs: list[str], region: str | None = None, exclude=(),
+                max_end: int | None = None):
     """The contigs a genome-wide call_variant processes, as (contig, start, end) intervals to tile with variant_intervals
     (ImageGenerationUI.generate_images, pepper_variant ImageGenerationUI.py:283-316): without `region`, every contig common to the
     FASTA and the BAM and not in `exclude`, in natural order, over [0, length - 1]; with it, the listed contigs in the listed order,
-    each span clamped to [0, length - 1]."""
+    each span clamped to [0, length - 1].  `max_end`: the BAM index's reach; a span that ends past it raises ValueError."""
     lengths = dict(fasta_contigs)
     if region is None:
         common = sorted((set(lengths) & set(bam_contigs)) - set(exclude), key=natural_key)
         if not common:
             raise ValueError("no contig common to the BAM and the FASTA")
-        return [(c, 0, lengths[c] - 1) for c in common]
-    job = []
-    for c, span in parse_region(region):
-        if c not in lengths:
-            raise ValueError("--region: contig %r is not in the FASTA" % c)
-        s, e = span if span is not None else (0, lengths[c] - 1)
-        job.append((c, max(0, s), min(e, lengths[c] - 1)))
+        job = [(c, 0, lengths[c] - 1) for c in common]
+    else:
+        job = []
+        for c, span in parse_region(region):
+            if c not in lengths:
+                raise ValueError("--region: contig %r is not in the FASTA" % c)
+            s, e = span if span is not None else (0, lengths[c] - 1)
+            job.append((c, max(0, s), min(e, lengths[c] - 1)))
+    check_reach([(c, e + 1) for c, _, e in job], max_end)
     return job
 
 
@@ -687,7 +713,7 @@ class PolishFileSource(_GroupSource):
     def __init__(self, bam_path: str, fasta_path: str, contigs: list[str] | None = None, device: int = 0, threads: int = 0,
                  gpu_inflate: bool = True, realign: bool = True, max_reads: int = POLISH_MAX_READS, host_share: float | None = None):
         super().__init__(bam_path, fasta_path, device, threads, gpu_inflate, host_share)
-        self._set_plan(*polish_job(self.fasta_contigs(), self.bam.get_chromosome_sequence_names(), contigs))
+        self._set_plan(*polish_job(self.fasta_contigs(), self.bam.get_chromosome_sequence_names(), contigs, self.bam.index_max_end))
         self.realign = realign
         self.realigner = Realigner(device) if realign else None
         self._max_reads = max_reads

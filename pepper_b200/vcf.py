@@ -358,10 +358,20 @@ def _bgzf(data: bytes, pool, level: int = 6):
     return b"".join(blocks) + BGZF_EOF, np.array(starts, np.int64), coff
 
 
+def vcf_csi_depth(fasta_contigs: list[tuple[str, int]], names: list[str]) -> int | None:
+    """None when every contig of `names` fits a TBI (shorter than 2^29, the reach of BAI binning); otherwise the depth of the CSI
+    that indexes the files instead: min_shift 14 and the smallest depth >= 5 that covers the longest contig (bcftools index)."""
+    from .synth_files import csi_depth_for, BAI_MAX_END
+    lengths = dict(fasta_contigs)
+    longest = max([lengths.get(n, 0) for n in names] + [0])
+    return None if longest <= BAI_MAX_END else csi_depth_for(longest)
+
+
 def _tabix(names: list[str], tids: np.ndarray, beg: np.ndarray, end: np.ndarray, ustart: np.ndarray, uend: np.ndarray,
-           blk_u: np.ndarray, blk_c: np.ndarray, eof_c: int, total_u: int) -> bytes:
+           blk_u: np.ndarray, blk_c: np.ndarray, eof_c: int, total_u: int, csi_depth: int | None = None) -> bytes:
     """TBI of a VCF (format 2, col_seq 1, col_beg 2, col_end 0, meta '#'): the per-reference bins / chunks / 16 kb linear index
-    are those of a BAI (synth_files._bai_bytes) over [pos, pos + len(REF)) and the lines' virtual offsets."""
+    are those of a BAI (synth_files._bai_bytes) over [pos, pos + len(REF)) and the lines' virtual offsets.  With `csi_depth`, a
+    CSI (min_shift 14) instead, whose aux holds the same configuration block, as `tabix --csi` writes; uncompressed either way."""
     blk_u, blk_c = np.asarray(blk_u, np.int64), np.asarray(blk_c, np.int64)
 
     def voff(u):
@@ -372,6 +382,14 @@ def _tabix(names: list[str], tids: np.ndarray, beg: np.ndarray, end: np.ndarray,
     beg, end = np.asarray(beg, np.int64), np.asarray(end, np.int64)
     vb, ve = voff(ustart), voff(uend)
     nm = b"".join(n.encode() + b"\0" for n in names)
+    if csi_depth is not None:
+        from .synth_files import csi_bytes, csi_reference
+        conf = struct.pack("<7i", 2, 1, 2, 0, ord("#"), 0, len(nm)) + nm
+        refs = []
+        for t in range(len(names)):
+            sel = np.flatnonzero(tids == t)
+            refs.append(csi_reference(beg[sel], end[sel], vb[sel], ve[sel], 14, csi_depth))
+        return csi_bytes(14, csi_depth, conf, refs)
     out = [b"TBI\x01" + struct.pack("<8i", len(names), 2, 1, 2, 0, ord("#"), 0, len(nm)) + nm]
     for t in range(len(names)):
         sel = np.flatnonzero(tids == t)
@@ -420,13 +438,15 @@ def _index_reference(beg: np.ndarray, end: np.ndarray, vb: np.ndarray, ve: np.nd
 def write_vcfs(out_dir: str, sample_name: str, fasta_contigs: list[tuple[str, int]], names: list[str], text: np.ndarray,
                lines: np.ndarray, threads: int = 8) -> tuple[int, int, int, int, int]:
     """Ordered lines (order_lines) -> the five bgzipped, tabix-indexed VCFs of write_vcf_records under `out_dir`; returns its
-    totals (full, pepper, variant calling, variant-calling SNPs, indels)."""
+    totals (full, pepper, variant calling, variant-calling SNPs, indels).  The index is a .tbi, or a .csi when a contig of `names`
+    is longer than 2^29 (vcf_csi_depth)."""
     import os
     from concurrent.futures import ThreadPoolExecutor
     os.makedirs(out_dir, exist_ok=True)
     head = vcf_header(sample_name, fasta_contigs).encode()
     cls = lines["cls"]
     masks = (np.ones(cls.shape[0], bool), cls == CLASS_PEPPER, cls != CLASS_PEPPER, cls == CLASS_VC_SNP, cls == CLASS_VC_INDEL)
+    depth = vcf_csi_depth(fasta_contigs, names)
     with ThreadPoolExecutor(max_workers=max(1, threads)) as pool:
         for name, mask in zip(VCF_FILES, masks):
             sel = lines[mask]
@@ -441,8 +461,8 @@ def write_vcfs(out_dir: str, sample_name: str, fasta_contigs: list[tuple[str, in
             tid_of = {c: i for i, c in enumerate(seen)}
             us = len(head) + np.concatenate([[0], np.cumsum(sel["text_len"].astype(np.int64))])
             tbi = _tabix([names[c] for c in seen], np.array([tid_of[c] for c in sel["contig"].tolist()], np.int64), sel["pos"],
-                         sel["pos"] + sel["ref_len"], us[:-1], us[1:], blk_u, blk_c, int(blk_c[-1]), len(data))
-            with open(path + ".tbi", "wb") as f:
+                         sel["pos"] + sel["ref_len"], us[:-1], us[1:], blk_u, blk_c, int(blk_c[-1]), len(data), depth)
+            with open(path + (".tbi" if depth is None else ".csi"), "wb") as f:
                 f.write(_bgzf(tbi, pool)[0])
     return tuple(int(m.sum()) for m in masks)
 
@@ -511,6 +531,7 @@ def write_vcfs_from_parts(out_dir: str, sample_name: str, fasta_contigs: list[tu
     head = vcf_header(sample_name, fasta_contigs).encode()
     lex = {c: i for i, c in enumerate(sorted(range(len(names)), key=lambda i: names[i]))}
     order = sorted(parts, key=lambda g: (lex[group_contig[g]], g))
+    depth = vcf_csi_depth(fasta_contigs, names)
     with ThreadPoolExecutor(max_workers=8) as pool:
         hgz, hu, hc = _bgzf(head, pool, 1)
         hgz = hgz[:-len(BGZF_EOF)]
@@ -536,8 +557,8 @@ def write_vcfs_from_parts(out_dir: str, sample_name: str, fasta_contigs: list[tu
             ul = cat(ulen, np.int64)
             us = len(head) + np.concatenate([[0], np.cumsum(ul)])
             tbi = _tabix([names[k] for k in seen], cat(tids, np.int64), cat(beg, np.int64), cat(end, np.int64), us[:-1], us[1:],
-                         np.concatenate(blk_u), np.concatenate(blk_c), c, u)
-            with open(path + ".tbi", "wb") as fh:
+                         np.concatenate(blk_u), np.concatenate(blk_c), c, u, depth)
+            with open(path + (".tbi" if depth is None else ".csi"), "wb") as fh:
                 fh.write(_bgzf(tbi, pool)[0])
 
 
