@@ -454,6 +454,12 @@ int pb_test_tc_gemm_ex(int M, int N, int epi, int K0, const float *h_A0, int lo0
  * (NULL = not written): h_y_f32 [M][33][512]; h_y_hi / h_y_lo [ceil(M / 128)][33][16][4096]; h_c_final [2][256][M].      */
 int pb_test_variant_lstm_layer(pb_variant_net_t *net, int layer, int M, const void *h_x, int lo_x, int lo_h, int persist,
                                int poison, float *h_y_f32, uint16_t *h_y_hi, uint16_t *h_y_lo, float *h_c_final);
+/* diagnostics: the int8-slice decoder LSTM layer of mode 2 (k_lstm_layer_q8).  h_x: fp32 [M][33][512], quantized on the host
+ * to the slices the encoder would write.  persist 0 = one launch per step.  Outputs (each may be NULL): y_f32 [M][33][512];
+ * h_q: the layer's own h slices, 2 x ceil(M / 128) x 33 x 8 x 8192 bytes (slice 1, then slice 0; tc_gemm.cuh QSeq layout);
+ * c_final [2][256][M].  poison: every buffer the launch touches starts as 0xff bytes. */
+int pb_test_variant_lstm_q8(pb_variant_net_t *net, int M, const float *h_x, int persist, int poison, float *h_y_f32, int8_t *h_q,
+                            float *h_c_final);
 /* diagnostics: one bidirectional GRU layer (0 encoder, 1 decoder) of a polish network over one 100-step window on the wgmma
  * path.  h_x: uint8 [M][100][10] or fp32 [M][100][256]; h_h0: [2][M][128] or NULL (zero state).  Output: the sequence tiles
  * h_y_hi / h_y_lo [ceil(M / 128)][100][8][4096] (direction d of step t in k-tiles 8 t + 4 d .. 8 t + 4 d + 3).         */

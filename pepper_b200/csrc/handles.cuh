@@ -11,10 +11,16 @@ struct DevLin { DevBuf W, bias; int N, K, Kp; };
 // `scale`: the power of two s the tiles hold s W in (max |s W| in (1/2, 1]); the epilogues multiply by 1 / s
 struct TcRnn { DevBuf w_hi, w_lo; int nkt_x = 0, nkt_h = 0; float scale = 1.f; };
 struct TcLin { DevBuf w_hi, w_lo; int nkt = 0; float scale = 1.f; };
+// int8-slice decoder layer (mode 2, tc_gemm.cuh k_lstm_layer_q8): the two slices of round(sw_n W[n][k]), sw_n = 32512 /
+// max_k |W[n][k]| over K = [W_ih | W_hh], as [8 n-tiles][12 k-tiles][128][64] byte images, and the epilogue's
+// 256 / (32512 sw_n) per gate column n
+struct TcRnnQ { DevBuf w1, w0, col_scale; };
 struct TcVariant {
     TcRnn enc[2], dec[2];
     TcLin lin[5];
-    DevBuf img_op, yenc_hi, yenc_lo, ydec_hi, ydec_lo, c, act_hi[2], act_lo[2], final_f32;
+    TcRnnQ decq[2];
+    // mode 2: the encoder writes the decoder's x slices (q1 | q0) into yenc_lo, the decoder its own h slices into ydec_q
+    DevBuf img_op, yenc_hi, yenc_lo, ydec_hi, ydec_lo, ydec_q, c, act_hi[2], act_lo[2], final_f32;
     // which GEMMs execute the third (a_lo x w_hi) product: bit 0 encoder h-part, 1 decoder x-part, 2 decoder h-part, 3 linear_1,
     // 4 linear_2..5; clearing a bit runs that GEMM with two products, 0x1f = three everywhere.  Default 0x1a: the recurrent
     // (h-part) GEMMs of both LSTM layers run with two products — each passes the parity gate on its own (hidden states within
@@ -59,6 +65,7 @@ struct PolishStream;       // streaming polish session state (pipeline.cu)
 void polish_stream_free(PolishStream *S);
 int tc_upload_rnn(TcRnn &T, const float *Wp, int K0, int K0p_src, int H, int Kp_src);
 int tc_upload_lin(TcLin &T, const float *w, int N, int K);
+int tc_upload_rnn_q8(TcRnnQ &T, const float *Wp, int K0, int K0p_src, int H, int Kp_src);
 }  // namespace pb
 
 struct pb_variant_encoder {
@@ -111,7 +118,7 @@ struct pb_polish_encoder {
 
 struct pb_variant_net {
     int device = 0;
-    int mode = 1;          // 1 = tensor-core hi/lo x3 (default), 0 = fp32 FFMA
+    int mode = 2;          // 2 = tensor cores, int8-slice decoder LSTM (default), 1 = tensor-core hi/lo x3, 0 = fp32 FFMA
     pb::TcVariant *tc = nullptr;
     pb::DevRnn enc[2], dec[2];
     pb::DevLin lin[5], outl;

@@ -393,6 +393,7 @@ extern "C" int pb_variant_net_create(pb_variant_net_t **out, int device, const f
         PB_TRY(upload_rnn(N->dec[d], pd));
         PB_TRY(tc_upload_rnn(N->tc->enc[d], pe.W.data(), pe.K0, pe.K0p, VH, pe.Kp));
         PB_TRY(tc_upload_rnn(N->tc->dec[d], pd.W.data(), pd.K0, pd.K0p, VH, pd.Kp));
+        PB_TRY(tc_upload_rnn_q8(N->tc->decq[d], pd.W.data(), pd.K0, pd.K0p, VH, pd.Kp));
     }
     PB_TRY(upload_lin(N->lin[0], P[16], P[17], 512, VT * 512));
     PB_TRY(tc_upload_lin(N->tc->lin[0], P[16], 512, VT * 512));
@@ -415,8 +416,9 @@ extern "C" int pb_variant_net_destroy(pb_variant_net_t *N) {
     if (N->tc) {
         TcVariant &T = *N->tc;
         for (int d = 0; d < 2; d++) { T.enc[d].w_hi.release(); T.enc[d].w_lo.release(); T.dec[d].w_hi.release(); T.dec[d].w_lo.release(); }
+        for (int d = 0; d < 2; d++) { T.decq[d].w1.release(); T.decq[d].w0.release(); T.decq[d].col_scale.release(); }
         for (auto &l : T.lin) { l.w_hi.release(); l.w_lo.release(); }
-        DevBuf *tb[] = {&T.img_op, &T.yenc_hi, &T.yenc_lo, &T.ydec_hi, &T.ydec_lo, &T.c, &T.act_hi[0], &T.act_hi[1], &T.act_lo[0], &T.act_lo[1], &T.final_f32};
+        DevBuf *tb[] = {&T.img_op, &T.yenc_hi, &T.yenc_lo, &T.ydec_hi, &T.ydec_lo, &T.ydec_q, &T.c, &T.act_hi[0], &T.act_hi[1], &T.act_lo[0], &T.act_lo[1], &T.final_f32};
         for (auto *b : tb) b->release();
         delete N->tc;
     }
@@ -426,14 +428,19 @@ extern "C" int pb_variant_net_destroy(pb_variant_net_t *N) {
 
 extern "C" int pb_variant_net_set_mode(pb_variant_net_t *N, int mode) {
     if (!N) return PB_ERR_ARG;
-    if (mode != 0 && mode != 1) { set_error("mode %d unknown (0 = fp32 FFMA, 1 = tensor-core hi/lo x3)", mode); return PB_ERR_ARG; }
+    if (mode < 0 || mode > 2) {
+        set_error("mode %d unknown (0 = fp32 FFMA, 1 = tensor-core hi/lo x3, 2 = tensor cores with the int8-slice decoder LSTM)", mode);
+        return PB_ERR_ARG;
+    }
     N->mode = mode;
     return PB_OK;
 }
-// experiments (DESIGN.md "two-product variant"): which GEMMs keep the third tensor-core product
+// experiments (DESIGN.md "two-product variant"): which GEMMs keep the third tensor-core product.  The mask selects among the
+// fp16 split's products, so a network in mode 2 goes back to mode 1, where every bit applies.
 extern "C" int pb_variant_net_set_lo_mask(pb_variant_net_t *N, int mask) {
     if (!N || !N->tc) { set_error("no tensor-core state"); return PB_ERR_ARG; }
     N->tc->lo_mask = mask & 0x1f;
+    if (N->mode == 2) N->mode = 1;
     return PB_OK;
 }
 extern "C" int pb_polish_net_set_lo_mask(pb_polish_net_t *N, int mask) {

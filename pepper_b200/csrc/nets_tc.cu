@@ -1,4 +1,4 @@
-// Host side of the tensor-core (wgmma) network path (mode 1): weight / operand tiling, per-layer launch sequences, and a
+// Host side of the tensor-core (wgmma) network paths (modes 1 and 2): weight / operand tiling, per-layer launch sequences, and a
 // GEMM self-test entry point.  Device code: tc_gemm.cuh.
 #include "handles.cuh"
 #include "tc_gemm.cuh"
@@ -90,6 +90,45 @@ int tc_upload_lin(TcLin &T, const float *w, int N, int K) {
     return upload_tiles(T.w_hi, T.w_lo, hi, lo);
 }
 
+// 16-bit fixed point q = rint(v * s) as two int8 slices q = 256 q1 + q0 (tc_gemm.cuh, "int8-slice operands")
+static inline void qsplit(double v_times_s, int8_t &q1, int8_t &q0) {
+    const int q = (int) std::nearbyint(v_times_s);
+    const int hi = (q + 128) >> 8;
+    q1 = (int8_t) hi;
+    q0 = (int8_t) (q - 256 * hi);
+}
+// byte offset of element (r, k) in a [rt][kt][4][128][16] slice image with KT k-tiles of 64 per row tile
+static inline int64_t qtiled_index(int64_t r, int64_t k, int64_t KT) {
+    return ((r / 128) * KT + k / 64) * tc::QTILE_BYTES + ((k % 64) / 16) * 2048 + (r % 128) * 16 + (k % 16);
+}
+
+// the decoder direction's weights for k_lstm_layer_q8: rows 4j+g of Wp [4H][Kp_src] with K = [x | pad32 | h] -> K = [x | h]
+int tc_upload_rnn_q8(TcRnnQ &T, const float *Wp, int K0, int K0p_src, int H, int Kp_src) {
+    if (K0 % tc::QK || H % tc::QK || 4 * H % tc::QN) { set_error("int8 LSTM packing needs K0, H %% 64 == 0"); return PB_ERR_ARG; }
+    const int K = K0 + H, N = 4 * H, KT = K / tc::QK;
+    std::vector<int8_t> w1((size_t) N * K), w0((size_t) N * K);
+    std::vector<float> cs(N);
+    for (int n = 0; n < N; n++) {
+        const float *x = Wp + (size_t) n * Kp_src, *h = x + K0p_src;
+        double m = 0.0;
+        for (int k = 0; k < K0; k++) m = std::max(m, (double) std::fabs(x[k]));
+        for (int k = 0; k < H; k++) m = std::max(m, (double) std::fabs(h[k]));
+        const double sw = m > 0.0 && std::isfinite(m) ? tc::QSCALE / m : 1.0;
+        cs[n] = (float) (256.0 / (tc::QSCALE * sw));
+        for (int k = 0; k < K; k++) {
+            const int64_t o = qtiled_index(n, k, KT);
+            qsplit((double) (k < K0 ? x[k] : h[k - K0]) * sw, w1[(size_t) o], w0[(size_t) o]);
+        }
+    }
+    PB_TRY(T.w1.reserve(w1.size()));
+    PB_TRY(T.w0.reserve(w0.size()));
+    PB_TRY(T.col_scale.reserve(sizeof(float) * N));
+    PB_CUDA(cudaMemcpy(T.w1.p, w1.data(), w1.size(), cudaMemcpyHostToDevice));
+    PB_CUDA(cudaMemcpy(T.w0.p, w0.data(), w0.size(), cudaMemcpyHostToDevice));
+    PB_CUDA(cudaMemcpy(T.col_scale.p, cs.data(), sizeof(float) * N, cudaMemcpyHostToDevice));
+    return PB_OK;
+}
+
 static int g_num_sms = 0;
 
 // persistent 128x256-tile kernel (weights packed in 256-row tiles); `nt128` = number of 128-column tiles = N / 128.
@@ -121,6 +160,9 @@ static Dir empty_dir() {
 
 // ------------------------------------------------------------------------------------------------- variant
 constexpr int VT = 33, VH = 256;
+// bytes per row tile of one slice of a 512-feature sequence (tc_gemm.cuh QSeq): 33 steps x 8 k-tiles.  Both slices of a
+// sequence take as many bytes as its fp16 lo tiles, so the encoder's go into T.yenc_lo (q1, then q0 at Mt * q_mt_bytes()).
+static constexpr int64_t q_mt_bytes() { return (int64_t) VT * 8 * tc::QTILE_BYTES; }
 
 #ifdef PB_LSTM_TRACE
 // Timing build only: the stamps of the latest launch of each variant LSTM layer (layer 0 words, then layer 1), on the
@@ -143,9 +185,10 @@ extern "C" int pb_lstm_trace_copy(uint64_t *host, int64_t n_words) {
 // One bidirectional LSTM layer of the variant network over its 33 steps, reading T.img_op (layer 0) or T.yenc (layer 1)
 // and writing T.yenc / T.ydec (+ the optional fp32 copy y_f32 [B][33][512]); the cell state ends in T.c.  lo_x / lo_h:
 // the a_lo x w_hi product of the x-part / h-part runs (the int8 images of layer 0 have no lo operand).  persist: one
-// k_lstm_layer launch, or 33 launches of the per-step k_tc_gemm_p<EPI_LSTM> cross-check path.
+// k_lstm_layer launch, or 33 launches of the per-step k_tc_gemm_p<EPI_LSTM> cross-check path.  q8 (layer 0, persistent
+// only): the layer writes the int8 slices of h for k_lstm_layer_q8 into T.yenc_lo instead of the fp16 lo tiles.
 static int variant_lstm_layer_tc(pb_variant_net *N, int layer, int64_t B, bool lo_x, bool lo_h, bool persist, float *y_f32,
-                                 cudaStream_t st) {
+                                 cudaStream_t st, bool q8 = false) {
     TcVariant &T = *N->tc;
     const int64_t Mt = ceil_div(B, 128), Bp = Mt * 128;
     PB_CUDA(cudaMemsetAsync(T.c.p, 0, sizeof(float) * 2 * VH * Bp, st));
@@ -174,19 +217,26 @@ static int variant_lstm_layer_tc(pb_variant_net *N, int layer, int64_t B, bool l
         if (y_f32) { L.y_f32 = y_f32; L.ldy = (int64_t) VT * 512; }
         L.M = (int) B; L.n_mt = (int) Mt; L.T = VT; L.c_ld = Bp;
         L.lo_x = lo_x; L.lo_h = lo_h;
+        if (q8) {
+            if (layer != 0 || lo_h) { set_error("int8 slice output: encoder layer with a hi-only h-part"); return PB_ERR_STATE; }
+            L.q1 = T.yenc_lo.as<int8_t>(); L.q0 = L.q1 + Mt * q_mt_bytes(); L.q_mt_stride = q_mt_bytes();
+        }
 #ifdef PB_LSTM_TRACE
         PB_TRY(lstm_trace_buffer(layer, &L.trace));
         PB_CUDA(cudaMemsetAsync(L.trace, 0, sizeof(uint64_t) * tc::lstm_trace_words(VT), st));
 #endif
         static bool attr_set = false;
         if (!attr_set) {
-            PB_CUDA(cudaFuncSetAttribute(tc::k_lstm_layer, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::LSTM_SMEM_BYTES));
+            PB_CUDA(cudaFuncSetAttribute(tc::k_lstm_layer<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::LSTM_SMEM_BYTES));
+            PB_CUDA(cudaFuncSetAttribute(tc::k_lstm_layer<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::LSTM_SMEM_BYTES));
             attr_set = true;
         }
-        tc::k_lstm_layer<<<(unsigned) (2 * Mt), tc::LSTM_THREADS, tc::LSTM_SMEM_BYTES, st>>>(L);
+        if (q8) tc::k_lstm_layer<true><<<(unsigned) (2 * Mt), tc::LSTM_THREADS, tc::LSTM_SMEM_BYTES, st>>>(L);
+        else tc::k_lstm_layer<false><<<(unsigned) (2 * Mt), tc::LSTM_THREADS, tc::LSTM_SMEM_BYTES, st>>>(L);
         N->launches++;
         return PB_OK;
     }
+    if (q8) { set_error("int8 slice output needs the persistent encoder kernel"); return PB_ERR_STATE; }
     for (int t = 0; t < VT; t++) {
         Args A;
         A.M = (int) B; A.N = 4 * VH; A.c_ld = Bp;
@@ -214,6 +264,40 @@ static int variant_lstm_layer_tc(pb_variant_net *N, int layer, int64_t B, bool l
     return PB_OK;
 }
 
+// The int8-slice decoder layer (mode 2): x = the encoder's slices in T.yenc_lo, h slices in T.ydec_q, fp16 hi / lo output
+// tiles in T.ydec_hi / T.ydec_lo for linear_1 (+ the optional fp32 copy).  persist: one k_lstm_layer_q8 launch for all 33
+// steps, or one launch per step (cross-check of the in-kernel h hand-off).
+static int variant_dec_q8(pb_variant_net *N, int64_t B, bool persist, float *y_f32, cudaStream_t st) {
+    TcVariant &T = *N->tc;
+    const int64_t Mt = ceil_div(B, 128), Bp = Mt * 128;
+    PB_CUDA(cudaMemsetAsync(T.c.p, 0, sizeof(float) * 2 * VH * Bp, st));
+    tc::LstmLayerQ L;
+    memset(&L, 0, sizeof(L));
+    L.x1 = T.yenc_lo.as<int8_t>(); L.x0 = L.x1 + Mt * q_mt_bytes();
+    L.q1 = T.ydec_q.as<int8_t>(); L.q0 = L.q1 + Mt * q_mt_bytes();
+    L.q_mt_stride = q_mt_bytes();
+    for (int d = 0; d < 2; d++) {
+        L.w1[d] = T.decq[d].w1.as<int8_t>(); L.w0[d] = T.decq[d].w0.as<int8_t>();
+        L.bias[d] = N->dec[d].bias.as<float>();
+        L.col_scale[d] = T.decq[d].col_scale.as<float>();
+        L.c[d] = T.c.as<float>() + (int64_t) d * VH * Bp;
+    }
+    L.y_hi = T.ydec_hi.as<bf16>(); L.y_lo = T.ydec_lo.as<bf16>(); L.y_mt_stride = (int64_t) VT * 16 * TILE_ELEMS;
+    if (y_f32) { L.y_f32 = y_f32; L.ldy = (int64_t) VT * 512; }
+    L.M = (int) B; L.n_mt = (int) Mt; L.T = VT; L.c_ld = Bp;
+    static bool attr_set = false;
+    if (!attr_set) {
+        PB_CUDA(cudaFuncSetAttribute(tc::k_lstm_layer_q8, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::QSMEM_BYTES));
+        attr_set = true;
+    }
+    for (int t0 = 0; t0 < VT; t0 = L.t1) {
+        L.t0 = t0; L.t1 = persist ? VT : t0 + 1;
+        tc::k_lstm_layer_q8<<<(unsigned) (2 * Mt), tc::LSTM_THREADS, tc::QSMEM_BYTES, st>>>(L);
+        N->launches++;
+    }
+    return PB_OK;
+}
+
 // scratch of one chunk of B candidates
 static int variant_reserve_tc(TcVariant &T, int64_t B) {
     const int64_t Mt = ceil_div(B, 128), Bp = Mt * 128;
@@ -223,6 +307,7 @@ static int variant_reserve_tc(TcVariant &T, int64_t B) {
     PB_TRY(T.yenc_lo.reserve((size_t) (seq_tiles * TILE_ELEMS) * 2));
     PB_TRY(T.ydec_hi.reserve((size_t) (seq_tiles * TILE_ELEMS) * 2));
     PB_TRY(T.ydec_lo.reserve((size_t) (seq_tiles * TILE_ELEMS) * 2));
+    PB_TRY(T.ydec_q.reserve((size_t) (2 * Mt * q_mt_bytes())));
     PB_TRY(T.c.reserve(sizeof(float) * 2 * VH * Bp));
     for (int i = 0; i < 2; i++) {
         PB_TRY(T.act_hi[i].reserve((size_t) (Mt * 16 * TILE_ELEMS) * 2));
@@ -244,8 +329,15 @@ int variant_forward_tc(pb_variant_net *N, const int8_t *d_images, int64_t B, flo
 
     // PB_LSTM_PERSIST=0 selects the per-step cross-check path
     static const bool persist = !(getenv("PB_LSTM_PERSIST") && atoi(getenv("PB_LSTM_PERSIST")) == 0);
-    PB_TRY(variant_lstm_layer_tc(N, 0, B, true, T.lo_mask & 1, persist, nullptr, st));
-    PB_TRY(variant_lstm_layer_tc(N, 1, B, (T.lo_mask >> 1) & 1, (T.lo_mask >> 2) & 1, persist, d_hidden_dbg, st));
+    if (N->mode == 2) {
+        // int8-slice decoder: the encoder runs its h-part hi only and hands the decoder its h as slices; lo_mask bits 0-2 do not
+        // apply (set_lo_mask returns the network to mode 1)
+        PB_TRY(variant_lstm_layer_tc(N, 0, B, true, false, true, nullptr, st, true));
+        PB_TRY(variant_dec_q8(N, B, persist, d_hidden_dbg, st));
+    } else {
+        PB_TRY(variant_lstm_layer_tc(N, 0, B, true, T.lo_mask & 1, persist, nullptr, st));
+        PB_TRY(variant_lstm_layer_tc(N, 1, B, (T.lo_mask >> 1) & 1, (T.lo_mask >> 2) & 1, persist, d_hidden_dbg, st));
+    }
     // MLP head
     for (int i = 0; i < 5; i++) {
         Args A;
@@ -582,6 +674,44 @@ extern "C" int pb_test_variant_lstm_layer(pb_variant_net_t *net, int layer, int 
         PB_CUDA(cudaMemcpy(h_y_hi, (layer == 0 ? T.yenc_hi : T.ydec_hi).p, (size_t) seq * 2, cudaMemcpyDeviceToHost));
         PB_CUDA(cudaMemcpy(h_y_lo, (layer == 0 ? T.yenc_lo : T.ydec_lo).p, (size_t) seq * 2, cudaMemcpyDeviceToHost));
     }
+    if (h_c_final)
+        for (int d = 0; d < 2; d++)
+            PB_CUDA(cudaMemcpy2D(h_c_final + (size_t) d * VH * M, sizeof(float) * M, T.c.as<float>() + (int64_t) d * VH * Bp,
+                                 sizeof(float) * Bp, sizeof(float) * M, VH, cudaMemcpyDeviceToHost));
+    return PB_OK;
+}
+
+// The int8-slice decoder layer (variant_dec_q8, the forward pass's own launch code) on host-quantized input slices.
+extern "C" int pb_test_variant_lstm_q8(pb_variant_net_t *net, int M, const float *h_x, int persist, int poison, float *h_y_f32, int8_t *h_q,
+                                       float *h_c_final) {
+    if (!net || !net->tc || M <= 0 || !h_x) { set_error("pb_test_variant_lstm_q8: bad argument"); return PB_ERR_ARG; }
+    PB_CUDA(cudaSetDevice(net->device));
+    TcVariant &T = *net->tc;
+    const int64_t Mt = ceil_div(M, 128), Bp = Mt * 128, qbytes = Mt * q_mt_bytes();
+    PB_TRY(variant_reserve_tc(T, M));
+    if (poison) {
+        DevBuf *bufs[] = {&T.yenc_lo, &T.ydec_hi, &T.ydec_lo, &T.ydec_q, &T.c};
+        for (auto *b : bufs) PB_TRY(fill_nan(*b));
+    }
+    // the encoder's quantization (tc_gemm.cuh qsplit2): rint(fp32(clamp(x, -1, 1) * 32512))
+    std::vector<int8_t> q(2 * qbytes, poison ? (int8_t) -1 : (int8_t) 0);
+    for (int64_t r = 0; r < M; r++)
+        for (int64_t k = 0; k < VT * 512; k++) {
+            const float v = std::min(std::max(h_x[r * VT * 512 + k], -1.f), 1.f) * tc::QSCALE;
+            const int64_t o = qtiled_index(r, k, VT * 8);
+            qsplit(v, q[o], q[qbytes + o]);
+        }
+    PB_CUDA(cudaMemcpy(T.yenc_lo.p, q.data(), q.size(), cudaMemcpyHostToDevice));
+    Scratch S;
+    if (h_y_f32) {
+        PB_TRY(S.b[0].reserve(sizeof(float) * (size_t) M * VT * 512));
+        PB_CUDA(cudaMemset(S.b[0].p, poison ? 0xff : 0, S.b[0].cap));
+    }
+    PB_TRY(variant_dec_q8(net, M, persist != 0, h_y_f32 ? S.b[0].as<float>() : nullptr, 0));
+    PB_CUDA(cudaGetLastError());
+    PB_CUDA(cudaDeviceSynchronize());
+    if (h_y_f32) PB_CUDA(cudaMemcpy(h_y_f32, S.b[0].p, sizeof(float) * (size_t) M * VT * 512, cudaMemcpyDeviceToHost));
+    if (h_q) PB_CUDA(cudaMemcpy(h_q, T.ydec_q.p, (size_t) (2 * qbytes), cudaMemcpyDeviceToHost));
     if (h_c_final)
         for (int d = 0; d < 2; d++)
             PB_CUDA(cudaMemcpy2D(h_c_final + (size_t) d * VH * M, sizeof(float) * M, T.c.as<float>() + (int64_t) d * VH * Bp,

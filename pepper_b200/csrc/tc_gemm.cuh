@@ -151,6 +151,52 @@ __device__ __forceinline__ void wgmma_256(float (&d)[128], uint64_t adesc, uint6
         : "l"(adesc), "l"(bdesc), "r"(1));
 }
 
+// ---------------------------------------------------------------- int8-slice operands (decoder LSTM layer, mode 2)
+// A value v in [-1, 1] (an LSTM hidden state) is held as the 16-bit fixed-point integer q = rint(v * 32512) split into two
+// signed int8 slices, q = 256 q1 + q0 with q1 = floor((q + 128) / 256) in [-127, 127] and q0 in [-128, 127].  A weight row
+// (gate column n, K = [W_ih | W_hh]) is held the same way at its own scale sw_n = 32512 / max_k |W[n][k]|.  Three s8 x s8
+// products with exact int32 accumulation, a1 w1 into acc_hh and a1 w0 + a0 w1 into acc_mix, give
+//   A W^T ~= (65536 acc_hh + 256 acc_mix) / (32512 sw_n)
+// dropping a0 w0 (<= 2^-16 of the product's range).  |acc_hh| <= 768 * 127^2 < 2^24 converts to fp32 exactly.
+// Tiled slice operand ("QSeq"): per (row tile, time step) 8 k-tiles of 128 rows x 64 k, one byte per element at
+// (k / 16) * 2048 + r * 16 + k % 16 (K-major no-swizzle canonical layout of 8-bit wgmma: core matrices 8 rows x 16 B, SBO
+// 128 B, LBO 2048 B); feature f of direction d is k = d * 256 + f.  Weight k-tiles have the same layout with 128 gate
+// columns for the 128 rows.
+constexpr int QK = 64;                              // k per ring stage
+constexpr int QTILE_BYTES = 128 * QK;               // 8 KB: one slice of a 128 x 64 tile
+constexpr int QN = 128;                             // gate columns per tile (32 hidden units x 4 gates)
+constexpr int QSTAGES = 6;
+constexpr int QSTAGE_BYTES = 4 * QTILE_BYTES;       // a1, a0, w1, w0 = 32 KB
+constexpr int QSMEM_BYTES = QSTAGES * QSTAGE_BYTES + 256 + 2 * 1024 * 4;   // ring + barriers + bias + column scales
+constexpr float QSCALE = 32512.f;
+
+// d[64 x 128] (s32) += A[64 x 32] B[128 x 32]^T, s8 operands K-major in shared memory
+__device__ __forceinline__ void wgmma_q8(int (&d)[64], uint64_t adesc, uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+          "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+          "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+          "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+          "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+          "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+          "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(1));
+}
+// u = q + 128 of a hidden value (the cell's h = sigm * tanh never leaves [-1, 1], so the clamp is the identity).  The slice
+// q1 = u >> 8 is byte 1 of u, and the byte of q0 = q - 256 q1 is byte 0 of u with its top bit flipped.
+__device__ __forceinline__ int qbias(float v) { return __float2int_rn(v * QSCALE) + 128; }
+// one slice (lo: q0, else q1) of four consecutive units, one byte each, from their qbias values
+__device__ __forceinline__ uint32_t qword(int u0, int u1, int u2, int u3, bool lo) {
+    const uint32_t sel = lo ? 0x40u : 0x51u;
+    const uint32_t w = __byte_perm(__byte_perm(u0, u1, sel), __byte_perm(u2, u3, sel), 0x5410);
+    return lo ? w ^ 0x80808080u : w;
+}
+
 // exp via ex2.approx (2 ulp) + fast divide: absolute error ~1e-6, far inside the 1e-3 parity tolerance.  exp_ftz is __expf
 // without its fix-up for results below 2^-126 (flushed to zero instead): the bits differ only where 1 + e rounds to 1
 // either way (sigm), and never occur in tanh_fast (e >= e^-30).
@@ -387,6 +433,8 @@ struct LstmLayer {
     int M, n_mt, T;
     int64_t c_ld;
     int lo_x, lo_h;                    // 1: the a_lo x w_hi product of the x-part / h-part is executed (0: two products)
+    int8_t *q1, *q0;                   // k_lstm_layer<true>: h_t as int8 slices for the next layer instead of y_lo (QSeq layout)
+    int64_t q_mt_stride;               // bytes
 #ifdef PB_LSTM_TRACE
     uint64_t *trace;                   // lstm_trace_words(T) stamps per launch, nullptr: none
 #endif
@@ -420,6 +468,9 @@ __device__ __forceinline__ uint64_t trace_gtime() {
 #define LSTM_STAMP(off) do {} while (0)
 #endif
 
+// Q8: the layer feeds the int8-slice decoder (mode 2).  The odd-unit lane writes h_t's two int8 slices to q1 / q0 instead of
+// the fp16 lo words, which nothing reads then (the layer's own h-part runs hi only): still 4 B per cell.
+template <bool Q8>
 __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
     extern __shared__ __align__(128) uint8_t smem[];
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem + PSTAGES * PSTAGE_BYTES);
@@ -515,14 +566,18 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
             // units nt * 64 .. + 63 are operand k-tiles 2 nt, 2 nt + 1 of this step.  Lanes q and q ^ 2 hold units 2 i and
             // 2 i + 1 of the same row: the even-unit lane writes the hi words of the pair, the odd-unit lane the lo words.
             const bool odd_u = q >> 1;
-            op_t *yw = (odd_u ? G.y_lo : G.y_hi) + y0 + 2 * nt * TILE_ELEMS;
+            op_t *yw = ((Q8 || !odd_u) ? G.y_hi : G.y_lo) + y0 + 2 * nt * TILE_ELEMS;
             float *yf = G.y_f32 ? G.y_f32 + (int64_t) row * G.ldy + (int64_t) tt * 512 + dir * 256 + nt * (PBN / 4) : nullptr;
+            // Q8: units nt * 64 .. + 63 are slice k-tile 4 dir + nt of this step
+            int8_t *qw = nullptr;
+            if constexpr (Q8) qw = (odd_u ? G.q0 : G.q1) + mt * G.q_mt_stride + (int64_t) (tt * 8 + dir * 4 + nt) * QTILE_BYTES + r128 * 16;
 #pragma unroll
             for (int m = 0; m < PBN / 16; m++) {
                 // cells i = 2 m, 2 m + 1: their two 4 B operand words are adjacent in row r128 and go out as one 8 B store
                 // (lanes 4 apart fill the other half of the 32 B sector); four cells per 16 B store need registers the
                 // 168-register launch does not have (68 B of spills)
                 uint32_t w[2];
+                int uq[4];
 #pragma unroll
                 for (int e = 0; e < 2; e++) {
                     const int i = 2 * m + e;
@@ -533,13 +588,24 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
                     if (valid) cp[i * c2s] = cn;
                     const float hp = __shfl_xor_sync(0xffffffffu, hn, 2);
                     const float h0 = odd_u ? hp : hn, h1 = odd_u ? hn : hp;          // units 2 i, 2 i + 1
-                    uint32_t hi, lo;
-                    split2<true>(h0, h1, hi, lo);
-                    w[e] = odd_u ? lo : hi;
+                    if constexpr (Q8) {
+                        uq[2 * e] = qbias(h0); uq[2 * e + 1] = qbias(h1);
+                        w[e] = (uint32_t) op_bits_unit(h0) | ((uint32_t) op_bits_unit(h1) << 16);
+                    } else {
+                        uint32_t hi, lo;
+                        split2<true>(h0, h1, hi, lo);
+                        w[e] = odd_u ? lo : hi;
+                    }
                     if (yf && valid && !odd_u) *reinterpret_cast<float2 *>(yf + 2 * i) = make_float2(h0, h1);
                 }
-                // element (unit nt * 64 + 4 m, row r128) of the step's operand tiles, relative to the lane's base
-                if (valid) __stwb(reinterpret_cast<uint2 *>(yw + (m >> 3) * TILE_ELEMS + ((m >> 1) & 3) * 1024 + 4 * (m & 1)), make_uint2(w[0], w[1]));
+                if constexpr (Q8) {
+                    // the even-unit lane writes the hi words and slice 1 of units nt * 64 + 4 m .. + 3, the odd-unit lane slice 0
+                    if (valid && !odd_u) __stwb(reinterpret_cast<uint2 *>(yw + (m >> 3) * TILE_ELEMS + ((m >> 1) & 3) * 1024 + 4 * (m & 1)), make_uint2(w[0], w[1]));
+                    if (valid) __stwb(reinterpret_cast<uint32_t *>(qw + (m >> 2) * 2048 + 4 * (m & 3)), qword(uq[0], uq[1], uq[2], uq[3], odd_u));
+                } else {
+                    // element (unit nt * 64 + 4 m, row r128) of the step's operand tiles, relative to the lane's base
+                    if (valid) __stwb(reinterpret_cast<uint2 *>(yw + (m >> 3) * TILE_ELEMS + ((m >> 1) & 3) * 1024 + 4 * (m & 1)), make_uint2(w[0], w[1]));
+                }
             }
             LSTM_STAMP(tc0 + 3);
         }
@@ -553,6 +619,182 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
 #ifdef PB_LSTM_TRACE
     if (tr && threadIdx.x == 0) { tr[147 * G.T + 2] = trace_gtime(); tr[147 * G.T + 3] = trace_clock(); }
 #endif
+}
+
+// ---------------------------------------------------------------- persistent LSTM decoder layer on int8 slices (variant, mode 2)
+// k_lstm_layer's structure (one CTA per (direction, row tile) for all steps, one producer thread streaming whole tiles onto an
+// mbarrier ring, h_t handed to the producer through bar_h) with int8-slice operands: K = [x (512) | h (256)] = 12 k-tiles of
+// 64, 128-column gate tiles (32 units x 4 gates, 8 per step) so that the two int32 accumulators of a warpgroup take the 128
+// registers one fp32 accumulator took.  Each step writes h_t as fp16 hi / lo operand tiles (linear_1) and as int8 slices (its
+// own h-part of the next step).  Steps t0 .. t1 - 1 run in one launch: the cell state and h stay in HBM between launches, so
+// one launch per step is the cross-check of the in-kernel hand-off.
+struct LstmLayerQ {
+    const int8_t *x1, *x0;             // input sequence slices (QSeq): tile (mt, tt, kt) at mt * q_mt_stride + (tt * 8 + kt) * QTILE_BYTES
+    const int8_t *w1[2], *w0[2];       // per direction: [8 n-tiles][12 k-tiles][QTILE_BYTES]
+    const float *bias[2];
+    const float *col_scale[2];         // [1024] 256 / (32512 sw_n)
+    float *c[2];                       // cell state per direction [256][c_ld]
+    int8_t *q1, *q0;                   // output sequence slices (QSeq); direction d -> k-tiles 4 d .. 4 d + 3
+    int64_t q_mt_stride;               // bytes, the same for x and q
+    op_t *y_hi, *y_lo;                 // output sequence operand [mt][T][16] fp16 tiles
+    int64_t y_mt_stride;
+    float *y_f32;                      // optional fp32 copy [row][T][512]
+    int64_t ldy;
+    int M, n_mt, T, t0, t1;
+    int64_t c_ld;
+};
+
+__device__ __forceinline__ void load_stage_q(uint32_t smem_base, uint32_t bar_full, uint32_t bar_empty, uint32_t g, const int8_t *a1,
+                                             const int8_t *a0, const int8_t *w1, const int8_t *w0) {
+    const uint32_t s = g % QSTAGES, ph = (g / QSTAGES) & 1u;
+    mbar_wait(bar_empty + 8 * s, ph ^ 1u);
+    const uint32_t st = smem_base + s * QSTAGE_BYTES;
+    mbar_expect_tx(bar_full + 8 * s, QSTAGE_BYTES);
+    bulk_g2s(st, a1, QTILE_BYTES, bar_full + 8 * s);
+    bulk_g2s(st + QTILE_BYTES, a0, QTILE_BYTES, bar_full + 8 * s);
+    bulk_g2s(st + 2 * QTILE_BYTES, w1, QTILE_BYTES, bar_full + 8 * s);
+    bulk_g2s(st + 3 * QTILE_BYTES, w0, QTILE_BYTES, bar_full + 8 * s);
+}
+
+__global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer_q8(LstmLayerQ G) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + QSTAGES * QSTAGE_BYTES);
+    float *sbias = reinterpret_cast<float *>(smem + QSTAGES * QSTAGE_BYTES + 256);
+    float *sscale = sbias + 1024;
+    const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + QSTAGES), bar_h = smem_u32(bars + 2 * QSTAGES);
+    const uint32_t smem_base = smem_u32(smem);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int dir = blockIdx.x / G.n_mt, mt = blockIdx.x % G.n_mt;
+    constexpr int X_NKT = 8, W_NKT = 12, N_TILES = 8;
+
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < QSTAGES; s++) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, CONS_WARPS); }
+        mbar_init(bar_h, CONS_WARPS);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    for (int i = threadIdx.x; i < 1024; i += LSTM_THREADS) { sbias[i] = G.bias[dir][i]; sscale[i] = G.col_scale[dir][i]; }
+    __syncthreads();
+
+    if (warp >= CONS_WARPS) {
+        reg_dealloc<LSTM_PROD_REGS>();
+        if (threadIdx.x == 32 * CONS_WARPS) {
+            uint32_t g = 0;
+            for (int t = G.t0; t < G.t1; t++) {
+                const int tt = dir ? G.T - 1 - t : t, tp = dir ? tt + 1 : tt - 1;
+                const int nkt = X_NKT + (t > 0 ? W_NKT - X_NKT : 0);
+                for (int nt = 0; nt < N_TILES; nt++) {
+                    for (int kt = 0; kt < nkt; kt++, g++) {
+                        const int8_t *a1, *a0;
+                        if (kt < X_NKT) {
+                            const int64_t off = (int64_t) mt * G.q_mt_stride + ((int64_t) tt * 8 + kt) * QTILE_BYTES;
+                            a1 = G.x1 + off; a0 = G.x0 + off;
+                        } else {
+                            if (kt == X_NKT && nt == 0 && t > G.t0) {
+                                // every consumer warp has written its part of h_{t-1}: make it visible to the bulk-copy engine
+                                mbar_wait(bar_h, (uint32_t) (t - G.t0 - 1) & 1u);
+                                asm volatile("fence.proxy.async;" ::: "memory");
+                            }
+                            const int64_t off = (int64_t) mt * G.q_mt_stride + ((int64_t) tp * 8 + dir * 4 + kt - X_NKT) * QTILE_BYTES;
+                            a1 = G.q1 + off; a0 = G.q0 + off;
+                        }
+                        const int64_t woff = ((int64_t) nt * W_NKT + kt) * QTILE_BYTES;
+                        load_stage_q(smem_base, bar_full, bar_empty, g, a1, a0, G.w1[dir] + woff, G.w0[dir] + woff);
+                    }
+                }
+            }
+        }
+        return;
+    }
+    reg_alloc<LSTM_CONS_REGS>();
+    const int wg = warp >> 2, q = lane & 3;
+    const int r128 = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * (q & 1);      // row of this lane's cells
+    const int row = mt * BM + r128;
+    const bool valid = row < G.M;
+    const bool odd_u = q >> 1;
+    const int c2 = 2 * (int) G.c_ld;
+    uint32_t g = 0;
+    int hh[64], mix[64];
+    for (int t = G.t0; t < G.t1; t++) {
+        const int tt = dir ? G.T - 1 - t : t;
+        const int nkt = X_NKT + (t > 0 ? W_NKT - X_NKT : 0);
+        for (int nt = 0; nt < N_TILES; nt++) {
+            float *cp = G.c[dir] + (int64_t) (nt * (QN / 4) + (q >> 1)) * G.c_ld + row;
+            float c_prev[QN / 8];
+#pragma unroll
+            for (int i = 0; i < QN / 8; i++) c_prev[i] = valid ? __ldcg(cp + i * c2) : 0.f;
+#pragma unroll
+            for (int i = 0; i < 64; i++) { hh[i] = 0; mix[i] = 0; }
+            for (int kt = 0; kt < nkt; kt++, g++) {
+                const uint32_t s = g % QSTAGES, ph = (g / QSTAGES) & 1u;
+                mbar_wait(bar_full + 8 * s, ph);
+                const uint32_t st = smem_base + s * QSTAGE_BYTES, a = st + (uint32_t) wg * 1024, b = st + 2 * QTILE_BYTES;
+                wg_fence();
+#pragma unroll
+                for (int ks = 0; ks < QK / 32; ks++) {
+                    const uint64_t a1 = smem_desc(a + ks * 4096, 2048), a0 = smem_desc(a + QTILE_BYTES + ks * 4096, 2048);
+                    const uint64_t w1 = smem_desc(b + ks * 4096, 2048), w0 = smem_desc(b + QTILE_BYTES + ks * 4096, 2048);
+                    wgmma_q8(hh, a1, w1);
+                    wgmma_q8(mix, a1, w0);
+                    wgmma_q8(mix, a0, w1);
+                }
+                wg_commit();
+                wg_wait<1>();
+                if (kt > 0) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(bar_empty + 8 * ((g - 1) % QSTAGES));
+                }
+            }
+            wg_wait<0>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(bar_empty + 8 * ((g - 1) % QSTAGES));
+
+            int c2s;
+            asm volatile("mov.b32 %0, %1;" : "=r"(c2s) : "r"(c2));
+            const float *sb = sbias + nt * QN + 2 * q, *ss = sscale + nt * QN + 2 * q;
+            // units nt * 32 .. + 31: fp16 k-tile dir * 8 + nt, slice k-tile 4 dir + nt / 2 (chunks 2 (nt & 1), + 1).  The
+            // even-unit lane writes the hi words and slice 1 of a unit pair, the odd-unit lane the lo words and slice 0.
+            op_t *yw = (odd_u ? G.y_lo : G.y_hi) + (int64_t) mt * G.y_mt_stride + (int64_t) (tt * 16 + dir * 8 + nt) * TILE_ELEMS + r128 * 8;
+            int8_t *qw = (odd_u ? G.q0 : G.q1) + mt * G.q_mt_stride + (int64_t) (tt * 8 + dir * 4 + (nt >> 1)) * QTILE_BYTES +
+                         (nt & 1) * 2 * 2048 + r128 * 16;
+            float *yf = G.y_f32 ? G.y_f32 + (int64_t) row * G.ldy + (int64_t) tt * 512 + dir * 256 + nt * (QN / 4) : nullptr;
+#pragma unroll
+            for (int m = 0; m < QN / 16; m++) {
+                uint32_t w[2];
+                int uq[4];
+#pragma unroll
+                for (int e = 0; e < 2; e++) {
+                    const int i = 2 * m + e;
+                    // gate columns 8 i + 2 q + {0, 1} of rows rA, rA + 8 (accumulator fragment of gates4)
+                    const float2 bz = *reinterpret_cast<const float2 *>(sb + 8 * i), sz = *reinterpret_cast<const float2 *>(ss + 8 * i);
+                    float v[4];
+#pragma unroll
+                    for (int k = 0; k < 4; k++)
+                        v[k] = fmaf(fmaf((float) hh[4 * i + k], 256.f, (float) mix[4 * i + k]), (k & 1) ? sz.y : sz.x, (k & 1) ? bz.y : bz.x);
+                    const float r0 = __shfl_xor_sync(0xffffffffu, (q & 1) ? v[0] : v[2], 1);
+                    const float r1 = __shfl_xor_sync(0xffffffffu, (q & 1) ? v[1] : v[3], 1);
+                    const float gi = (q & 1) ? r0 : v[0], gf = (q & 1) ? r1 : v[1];
+                    const float gg = (q & 1) ? v[2] : r0, go = (q & 1) ? v[3] : r1;
+                    const float cn = sigm(gf) * c_prev[i] + sigm(gi) * tanh_fast(gg);
+                    const float hn = sigm(go) * tanh_fast(cn);
+                    if (valid) cp[i * c2s] = cn;
+                    const float hp = __shfl_xor_sync(0xffffffffu, hn, 2);
+                    const float h0 = odd_u ? hp : hn, h1 = odd_u ? hn : hp;          // units 2 i, 2 i + 1
+                    uint32_t hi, lo;
+                    split2<true>(h0, h1, hi, lo);
+                    w[e] = odd_u ? lo : hi;
+                    uq[2 * e] = qbias(h0); uq[2 * e + 1] = qbias(h1);
+                    if (yf && valid && !odd_u) *reinterpret_cast<float2 *>(yf + 2 * i) = make_float2(h0, h1);
+                }
+                // units nt * 32 + 4 m .. + 3 of row r128
+                if (valid) __stwb(reinterpret_cast<uint2 *>(yw + (m >> 1) * 1024 + 4 * (m & 1)), make_uint2(w[0], w[1]));
+                if (valid) __stwb(reinterpret_cast<uint32_t *>(qw + (m >> 2) * 2048 + 4 * (m & 3)), qword(uq[0], uq[1], uq[2], uq[3], odd_u));
+            }
+        }
+        // h_t of this warp's rows is complete (all eight gate tiles): publish it to the producer thread
+        __threadfence();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_h);
+    }
 }
 
 // ---------------------------------------------------------------- persistent GRU layer kernel (polish)

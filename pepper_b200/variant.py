@@ -189,13 +189,16 @@ class VariantNet:
         return (probs, hid) if return_hidden else probs
 
     def set_mode(self, mode: int) -> None:
-        """0 = fp32 FFMA GEMMs, 1 = wgmma GEMMs with the 16-bit hi/lo operand split (2-3 products per GEMM, set_lo_mask; default)."""
+        """0 = fp32 FFMA GEMMs, 1 = wgmma GEMMs with the 16-bit hi/lo operand split (2-3 products per GEMM, set_lo_mask),
+        2 = mode 1 with the decoder LSTM on int8 tensor cores: 16-bit fixed-point operands as two int8 slices, exact int32
+        accumulation (default; DESIGN.md section 4)."""
         _lib.check(self.L.pb_variant_net_set_mode(self.h, mode), "pb_variant_net_set_mode")
 
     def set_lo_mask(self, mask: int) -> None:
         """Bit set = that GEMM keeps its third tensor-core product (a_lo x w_hi).  bits: 0 encoder h-part, 1 decoder x-part,
         2 decoder h-part, 3 linear_1, 4 linear_2-5.  Default 0x1a: the recurrent GEMMs pass the parity gate with two products
-        (DESIGN.md section 4); 0x1f = three everywhere."""
+        (DESIGN.md section 4); 0x1f = three everywhere.  The bits select among the fp16 split's products, so calling this puts
+        a network in mode 2 back on mode 1."""
         self.L.pb_variant_net_set_lo_mask.argtypes = [C.c_void_p, C.c_int]
         _lib.check(self.L.pb_variant_net_set_lo_mask(self.h, mask), "pb_variant_net_set_lo_mask")
 

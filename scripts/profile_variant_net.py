@@ -5,7 +5,9 @@ Each k_lstm_layer CTA does the same work whatever the grid size, so a layer that
 than at 1,408 (22 CTAs) at the same clock is held back by something the CTAs share, such as L2 bandwidth for the weight tiles
 every CTA streams.
 
-    python scripts/profile_variant_net.py [--sizes 8448 1408] [--reps 5] [--out FILE]     (PB_LIB_PATH selects the build)
+    python scripts/profile_variant_net.py [--sizes 8448 1408] [--reps 5] [--mode 2] [--out FILE]     (PB_LIB_PATH selects the build)
+
+In mode 2 the decoder layer is k_lstm_layer_q8 (int8 slices); --mode 1 profiles the fp16 hi/lo decoder of the same build.
 """
 import argparse
 import json
@@ -66,6 +68,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--sizes", type=int, nargs="+", default=[8448, 1408])
     ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--mode", type=int, default=None, help="VariantNet.set_mode before profiling (default: the library's default)")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     from oracle import nets
@@ -74,8 +77,10 @@ def main():
     gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
                          text=True).stdout.strip()
     net = VariantNet(nets.make_variant_weights(0), 0)
+    if args.mode is not None:
+        net.set_mode(args.mode)
     rng = np.random.default_rng(0)
-    res = {"gpu": gpu, "lib": os.environ.get("PB_LIB_PATH", "in-tree"), "sizes": [profile_size(net, n, args.reps, rng) for n in args.sizes]}
+    res = {"gpu": gpu, "mode": args.mode, "lib": os.environ.get("PB_LIB_PATH", "in-tree"), "sizes": [profile_size(net, n, args.reps, rng) for n in args.sizes]}
     net.close()
     txt = json.dumps(res, indent=1)
     print(txt)

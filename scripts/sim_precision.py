@@ -4,7 +4,11 @@ Every GEMM of the two networks is re-evaluated with operands rounded the way a g
 wgmma.mma_async (fp32 accumulate; products of 16-bit operands are exact in fp32), and the hidden states / probabilities are
 compared with the fp32 CPU oracle.  Used to choose the scheme before spending GPU time; the GPU tests are the gate.
 
-    python scripts/sim_precision.py variant|polish [n]
+    python scripts/sim_precision.py variant|polish [n] [scheme,scheme,...]
+
+A variant scheme name ending in "+i8dec" runs the decoder LSTM on int8 slices (mode 2, k_lstm_layer_q8: 16-bit fixed-point
+activations at the fixed scale 32,512, one per-column weight scale over [W_ih | W_hh], a0 x w0 dropped) and every other GEMM
+with the scheme before it, e.g. "f16x3+i8dec".
 """
 import sys
 import os
@@ -27,12 +31,33 @@ def split(x, dt):
     return hi, lo
 
 
+def q16(x, scale):
+    """16-bit fixed point x * scale = 256 x1 + x0 as two int8 slices, x1 = floor((q + 128) / 256), x0 in [-128, 127]"""
+    xi = torch.round(x * scale)
+    x1 = torch.floor((xi + 128) / 256)
+    return x1, xi - 256 * x1
+
+
+def i8_joint(a, W, S):
+    """a [B, K] in [-1, 1] times W [N, K] on int8 slices with exact accumulation and the a0 x w0 product dropped"""
+    key = ("i8", id(W))
+    if key not in S.cache:
+        W64 = W.to(torch.float64)
+        sw = 32512.0 / W64.abs().amax(1, keepdim=True).clamp_min(1e-30)
+        S.cache[key] = (*q16(W64, sw), sw)
+    w1, w0, sw = S.cache[key]
+    a1, a0 = q16(a.clamp(-1, 1), 32512.0)
+    acc = a1 @ w1.T * 65536 + (a1 @ w0.T + a0 @ w1.T) * 256
+    return acc / 32512.0 / sw.T
+
+
 class Scheme:
     """mm(a, W) with a [B,K] float64 activations, W [N,K] weights (fp32 values)."""
 
     def __init__(self, name):
         self.name = name
         self.cache = {}
+        self.i8_dec = False
 
     def wsplit(self, W, dt, scale=True):
         key = (id(W), dt)
@@ -89,7 +114,13 @@ def lstm_dir(S, x, Wih, Whh, b, reverse, slots=(0, 0)):
     out = torch.zeros(B, T, H, dtype=torch.float64)
     ts = range(T - 1, -1, -1) if reverse else range(T)
     for t in ts:
-        g = S.mm(x[:, t], Wih, slot=slots[0]) + S.mm(h, Whh, slot=slots[1]) + b
+        if S.i8_dec and slots[0] == 1:
+            key = ("cat", id(Wih), id(Whh))
+            if key not in S.cache:
+                S.cache[key] = torch.cat([Wih, Whh], 1)
+            g = i8_joint(torch.cat([x[:, t].double(), h], 1), S.cache[key], S) + b
+        else:
+            g = S.mm(x[:, t], Wih, slot=slots[0]) + S.mm(h, Whh, slot=slots[1]) + b
         g = g.float()       # epilogue works in fp32
         i, f, gg, o = g.chunk(4, dim=1)
         c = (torch.sigmoid(f) * c.float() + torch.sigmoid(i) * torch.tanh(gg))
@@ -177,7 +208,8 @@ def main():
             x[rng.random((n, 33, 26)) < 0.5] = 0
             want, whid = nets.variant_predict(st, x, threads=8, return_hidden=True)
             for name in schemes:
-                S = Scheme(name)
+                S = Scheme(name.replace("+i8dec", ""))
+                S.i8_dec = name.endswith("+i8dec")
                 p, hid = variant_forward(S, st, torch.from_numpy(x.astype(np.float32)))
                 eh = np.abs(hid.numpy() - whid).max()
                 ep = np.abs(p.numpy() - want).max()
