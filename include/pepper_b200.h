@@ -397,8 +397,15 @@ int pb_variant_net_forward_host(pb_variant_net_t *net, const int8_t *h_images,
                                 int64_t n, float *h_probs, float *h_hidden_dbg,
                                 void *stream);
 /* GEMM path: 0 = fp32 FFMA (reference-exact ordering), 1 = wgmma with the fp16 hi/lo operand split (2-3 products per GEMM,
- * see pb_variant_net_set_lo_mask; default)                                                                                       */
+ * see pb_variant_net_set_lo_mask), 2 = mode 1 with the decoder LSTM on int8 tensor cores.  pb_variant_net_create picks 2 when
+ * the decoder's weights pass the int8 guard below, else 1; an explicit set_mode(2) is honoured either way.                     */
 int pb_variant_net_set_mode(pb_variant_net_t *net, int mode);
+/* The int8 guard.  gate_err: the largest, over the decoder's gate rows, of a weight-only estimate of the error mode 2's 16-bit
+ * weight slices (one scale per row, set by the row's largest |w|) and its dropped low x low product add to a gate
+ * pre-activation for activations in [-1, 1] (DESIGN.md "Int8-slice decoder").  A network is created in mode 2 only when it is
+ * below PB_VARIANT_Q8_MAX_GATE_ERR.  mode: the network's current mode.  Either pointer may be NULL.                           */
+#define PB_VARIANT_Q8_MAX_GATE_ERR 1e-4
+int pb_variant_net_q8_guard(pb_variant_net_t *net, double *gate_err, int *mode);
 int pb_variant_net_launches(pb_variant_net_t *net, int64_t *n_launches);
 
 /* ------------------------------------------------------------------------

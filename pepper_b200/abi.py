@@ -18,6 +18,9 @@ PB_ERR_CUDA = -2
 PB_ERR_CAPACITY = -3
 PB_ERR_STATE = -4
 
+# pb_variant_net_create runs the decoder in mode 2 only below this weight-only gate error estimate (pb_variant_net_q8_guard)
+PB_VARIANT_Q8_MAX_GATE_ERR = 1e-4
+
 
 class PbReads(C.Structure):
     _fields_ = [("n_reads", C.c_int64),

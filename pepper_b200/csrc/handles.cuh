@@ -8,13 +8,14 @@ struct VariantStream;      // streaming session state (pipeline.cu)
 struct DevRnn { DevBuf W, bias; int K0, K0p, K1, Kp, H; };
 struct DevLin { DevBuf W, bias; int N, K, Kp; };
 // tensor-core path (nets_tc.cu): weights as 16-bit hi/lo tile images + per-chunk tiled operands
-// `scale`: the power of two s the tiles hold s W in (max |s W| in (1/2, 1]); the epilogues multiply by 1 / s
+// `scale`: the power of two s the tiles hold s W in (max |s W| in (2^14, 2^15]); the epilogues multiply by 1 / s
 struct TcRnn { DevBuf w_hi, w_lo; int nkt_x = 0, nkt_h = 0; float scale = 1.f; };
 struct TcLin { DevBuf w_hi, w_lo; int nkt = 0; float scale = 1.f; };
 // int8-slice decoder layer (mode 2, tc_gemm.cuh k_lstm_layer_q8): the two slices of round(sw_n W[n][k]), sw_n = 32512 /
 // max_k |W[n][k]| over K = [W_ih | W_hh], as [8 n-tiles][12 k-tiles][128][64] byte images, and the epilogue's
-// 256 / (32512 sw_n) per gate column n
-struct TcRnnQ { DevBuf w1, w0, col_scale; };
+// 256 / (32512 sw_n) per gate column n.  gate_err: the largest weight-only estimate over the rows of the error the slices add to
+// a gate pre-activation (nets_tc.cu tc_upload_rnn_q8); pb_variant_net_create compares it with PB_VARIANT_Q8_MAX_GATE_ERR
+struct TcRnnQ { DevBuf w1, w0, col_scale; double gate_err = 0.0; };
 struct TcVariant {
     TcRnn enc[2], dec[2];
     TcLin lin[5];
@@ -118,7 +119,10 @@ struct pb_polish_encoder {
 
 struct pb_variant_net {
     int device = 0;
-    int mode = 2;          // 2 = tensor cores, int8-slice decoder LSTM (default), 1 = tensor-core hi/lo x3, 0 = fp32 FFMA
+    // 2 = tensor cores, int8-slice decoder LSTM, 1 = tensor-core hi/lo x3, 0 = fp32 FFMA.  pb_variant_net_create picks 2 when the
+    // decoder's weights pass the int8 guard (q8_gate_err < PB_VARIANT_Q8_MAX_GATE_ERR), else 1
+    int mode = 2;
+    double q8_gate_err = 0.0;
     pb::TcVariant *tc = nullptr;
     pb::DevRnn enc[2], dec[2];
     pb::DevLin lin[5], outl;

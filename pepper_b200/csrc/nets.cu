@@ -402,7 +402,20 @@ extern "C" int pb_variant_net_create(pb_variant_net_t **out, int device, const f
         PB_TRY(tc_upload_lin(N->tc->lin[i], P[16 + 2 * i], 512, 512));
     }
     PB_TRY(upload_lin(N->outl, P[26], P[27], 3, 512));
+    // the int8 guard: weights whose slices would cost a gate more than the threshold run the decoder on the fp16 split instead,
+    // with all three products: the two-product recurrent GEMMs of mask 0x1a miss the parity gate on such weights too (an
+    // outlier of 100 std in W_hh multiplies the dropped a_lo, DESIGN.md "Int8-slice decoder")
+    N->q8_gate_err = std::max(N->tc->decq[0].gate_err, N->tc->decq[1].gate_err);
+    N->mode = N->q8_gate_err < PB_VARIANT_Q8_MAX_GATE_ERR ? 2 : 1;
+    if (N->mode == 1) N->tc->lo_mask = 0x1f;
     *out = N;
+    return PB_OK;
+}
+
+extern "C" int pb_variant_net_q8_guard(pb_variant_net_t *N, double *gate_err, int *mode) {
+    if (!N) { set_error("null network"); return PB_ERR_ARG; }
+    if (gate_err) *gate_err = N->q8_gate_err;
+    if (mode) *mode = N->mode;
     return PB_OK;
 }
 

@@ -49,9 +49,10 @@ static int upload_tiles(DevBuf &dhi, DevBuf &dlo, const std::vector<uint16_t> &h
     return PB_OK;
 }
 
-// The power of two s with max |s W| in (1/2, 1].  An fp16 w_lo is subnormal below 2^-14, i.e. for |s w| < 2^-3, where it
-// carries an absolute error of up to 2^-25: scaled, that error is 2^-25 / s of the unscaled weight instead of 2^-25, so the
-// split of the small weights of a default-initialised layer (|w| <= 1/16 .. 1/130) keeps its 22 bits relative to the layer.
+// The power of two s with max |s W| in (2^14, 2^15] (fp16 holds up to 65,504).  An fp16 w_lo is subnormal below 2^-14, i.e.
+// for |s w| < 2^-3, where it carries an absolute error of up to 2^-25: scaled, that error is 2^-25 / s of the unscaled weight,
+// and the split keeps its 22 bits for every weight down to 2^-17 of the matrix maximum.  A heavy-tailed matrix (one weight
+// at 100x the std of the rest) needs that range: at max |s W| ~ 1, most of its weights' w_lo would be subnormal.
 static float pow2_scale(const float *w, size_t n) {
     float m = 0.f;
     for (size_t i = 0; i < n; i++) m = std::max(m, std::fabs(w[i]));
@@ -59,7 +60,7 @@ static float pow2_scale(const float *w, size_t n) {
     int e;
     const float f = std::frexp(m, &e);                      // m = f 2^e, f in [1/2, 1)
     e = std::min(std::max(f == 0.5f ? e - 1 : e, -60), 60); // ceil(log2 m)
-    return std::ldexp(1.f, -e);
+    return std::ldexp(1.f, 15 - e);
 }
 
 // weights of one RNN direction, packed rows 4j+g (host copy kept by nets.cu) with K = [x | pad32 | h]; x-part and h-part
@@ -102,12 +103,17 @@ static inline int64_t qtiled_index(int64_t r, int64_t k, int64_t KT) {
     return ((r / 128) * KT + k / 64) * tc::QTILE_BYTES + ((k % 64) / 16) * 2048 + (r % 128) * 16 + (k % 16);
 }
 
-// the decoder direction's weights for k_lstm_layer_q8: rows 4j+g of Wp [4H][Kp_src] with K = [x | pad32 | h] -> K = [x | h]
+// the decoder direction's weights for k_lstm_layer_q8: rows 4j+g of Wp [4H][Kp_src] with K = [x | pad32 | h] -> K = [x | h].
+// T.gate_err: the largest over rows n of the weight-only error estimate of DESIGN.md "Int8-slice decoder" (guard),
+//   e_n = sqrt(sum_k (w_k / sw_n - W_k)^2 + (128^2 / 3) / 32512^2 sum_k (w0_k / sw_n)^2)
+// (weight rounding at |a_k| = 1, plus the dropped a0 w0 product with a0 uniform over its 8 bits).
 int tc_upload_rnn_q8(TcRnnQ &T, const float *Wp, int K0, int K0p_src, int H, int Kp_src) {
     if (K0 % tc::QK || H % tc::QK || 4 * H % tc::QN) { set_error("int8 LSTM packing needs K0, H %% 64 == 0"); return PB_ERR_ARG; }
     const int K = K0 + H, N = 4 * H, KT = K / tc::QK;
+    const double a0_var = 128.0 * 128.0 / 3.0 / ((double) tc::QSCALE * tc::QSCALE);
     std::vector<int8_t> w1((size_t) N * K), w0((size_t) N * K);
     std::vector<float> cs(N);
+    T.gate_err = 0.0;
     for (int n = 0; n < N; n++) {
         const float *x = Wp + (size_t) n * Kp_src, *h = x + K0p_src;
         double m = 0.0;
@@ -115,10 +121,17 @@ int tc_upload_rnn_q8(TcRnnQ &T, const float *Wp, int K0, int K0p_src, int H, int
         for (int k = 0; k < H; k++) m = std::max(m, (double) std::fabs(h[k]));
         const double sw = m > 0.0 && std::isfinite(m) ? tc::QSCALE / m : 1.0;
         cs[n] = (float) (256.0 / (tc::QSCALE * sw));
+        double e_round = 0.0, e_drop = 0.0;
         for (int k = 0; k < K; k++) {
             const int64_t o = qtiled_index(n, k, KT);
-            qsplit((double) (k < K0 ? x[k] : h[k - K0]) * sw, w1[(size_t) o], w0[(size_t) o]);
+            const double w = k < K0 ? x[k] : h[k - K0];
+            int8_t &s1 = w1[(size_t) o], &s0 = w0[(size_t) o];
+            qsplit(w * sw, s1, s0);
+            const double r = (256.0 * s1 + s0) / sw - w, d = s0 / sw;
+            e_round += r * r;
+            e_drop += d * d;
         }
+        T.gate_err = std::max(T.gate_err, std::sqrt(e_round + a0_var * e_drop));
     }
     PB_TRY(T.w1.reserve(w1.size()));
     PB_TRY(T.w0.reserve(w0.size()));

@@ -6,7 +6,7 @@
 // accumulated into the same fp32 tile:  a*w ~= a_hi*w_hi + a_hi*w_lo + a_lo*w_hi.  This is not fp32-equivalent: measured on
 // H100 the wgmma accumulation error grows about linearly with K, and a layer's error against exact float64 is 2-5x that of a
 // float32 CPU layer (tests/test_tc_layers_gpu.py).  Each packed weight matrix is scaled by a
-// power of two s (max |s W| in (1/2, 1]) so that w_lo stays out of the fp16 subnormals for every weight within 2^-3 of
+// power of two s (max |s W| in (2^14, 2^15]) so that w_lo stays out of the fp16 subnormals for every weight within 2^-17 of
 // the matrix maximum; the epilogues undo s exactly (fmaf(acc, 1/s, bias)).
 //
 // Every operand lives in HBM already in the shared-memory image of its tile ("tiled operand": for a tile of 128

@@ -191,8 +191,26 @@ class VariantNet:
     def set_mode(self, mode: int) -> None:
         """0 = fp32 FFMA GEMMs, 1 = wgmma GEMMs with the 16-bit hi/lo operand split (2-3 products per GEMM, set_lo_mask),
         2 = mode 1 with the decoder LSTM on int8 tensor cores: 16-bit fixed-point operands as two int8 slices, exact int32
-        accumulation (default; DESIGN.md section 4)."""
+        accumulation (DESIGN.md section 4).  A new network is in mode 2 when its decoder weights pass the int8 guard
+        (`q8_gate_err`), else in mode 1; setting a mode here overrides that choice."""
         _lib.check(self.L.pb_variant_net_set_mode(self.h, mode), "pb_variant_net_set_mode")
+
+    def _q8_guard(self) -> tuple[float, int]:
+        err, mode = C.c_double(0.0), C.c_int(0)
+        self.L.pb_variant_net_q8_guard.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int)]
+        _lib.check(self.L.pb_variant_net_q8_guard(self.h, C.byref(err), C.byref(mode)), "pb_variant_net_q8_guard")
+        return float(err.value), int(mode.value)
+
+    @property
+    def mode(self) -> int:
+        """the mode the next predict runs in"""
+        return self._q8_guard()[1]
+
+    @property
+    def q8_gate_err(self) -> float:
+        """weight-only estimate of the error the int8 decoder adds to a gate pre-activation (largest over gate rows); the
+        network was created in mode 2 only if it is below abi.PB_VARIANT_Q8_MAX_GATE_ERR"""
+        return self._q8_guard()[0]
 
     def set_lo_mask(self, mask: int) -> None:
         """Bit set = that GEMM keeps its third tensor-core product (a_lo x w_hi).  bits: 0 encoder h-part, 1 decoder x-part,

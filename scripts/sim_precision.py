@@ -4,12 +4,16 @@ Every GEMM of the two networks is re-evaluated with operands rounded the way a g
 wgmma.mma_async (fp32 accumulate; products of 16-bit operands are exact in fp32), and the hidden states / probabilities are
 compared with the fp32 CPU oracle.  Used to choose the scheme before spending GPU time; the GPU tests are the gate.
 
-    python scripts/sim_precision.py variant|polish [n] [scheme,scheme,...]
+    python scripts/sim_precision.py variant|polish [n] [scheme,scheme,...] [--weights uniform|t3|outlier30|outlier100]
+
+--weights (variant only) replaces the decoder LSTM's weights, at each matrix's std, with Student-t (3 dof) samples or puts one
+weight per gate row at +-30 / +-100 std (tests/test_weight_distributions_gpu.py builds the same states for the GPU).
 
 A variant scheme name ending in "+i8dec" runs the decoder LSTM on int8 slices (mode 2, k_lstm_layer_q8: 16-bit fixed-point
 activations at the fixed scale 32,512, one per-column weight scale over [W_ih | W_hh], a0 x w0 dropped) and every other GEMM
 with the scheme before it, e.g. "f16x3+i8dec".
 """
+import argparse
 import sys
 import os
 import numpy as np
@@ -195,13 +199,39 @@ def polish_forward(S, st, images):
     return acc.numpy(), np.stack(hids)
 
 
+def reweight_decoder(st, dist, seed):
+    """the decoder's W_ih / W_hh replaced as --weights says (uniform: unchanged)"""
+    if dist == "uniform":
+        return st
+    st = dict(st)
+    rng = np.random.default_rng([seed, 1])
+    for suf in ("", "_reverse"):
+        for i, part in enumerate(("ih", "hh")):
+            name = f"decoder.weight_{part}_l0{suf}"
+            W = st[name].numpy().astype(np.float64)
+            if dist == "t3":
+                X = rng.standard_t(3, size=W.shape)
+                W = X * (W.std() / X.std())
+            else:                 # outlier30 / outlier100: W_ih holds the even rows' outliers, W_hh the odd rows'
+                k = float(dist[len("outlier"):])
+                rows = np.arange(i, W.shape[0], 2)
+                W = W.copy()
+                W[rows, rng.integers(0, W.shape[1], rows.size)] = k * W.std() * rng.choice([-1.0, 1.0], rows.size)
+            st[name] = torch.from_numpy(W.astype(np.float32))
+    return st
+
+
 def main():
-    which = sys.argv[1]
-    n = int(sys.argv[2]) if len(sys.argv) > 2 else 256
-    schemes = sys.argv[3].split(",") if len(sys.argv) > 3 else ["bf16x3", "f16x3", "f16x2", "f16x2a", "f16x1", "bf16x2"]
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("which", choices=["variant", "polish"])
+    ap.add_argument("n", type=int, nargs="?", default=256)
+    ap.add_argument("schemes", nargs="?", default="bf16x3,f16x3,f16x2,f16x2a,f16x1,bf16x2")
+    ap.add_argument("--weights", choices=["uniform", "t3", "outlier30", "outlier100"], default="uniform")
+    args = ap.parse_args()
+    which, n, schemes, dist = args.which, args.n, args.schemes.split(","), args.weights
     if which == "variant":
         for seed in (1, 2):
-            st = nets.make_variant_weights(seed)
+            st = reweight_decoder(nets.make_variant_weights(seed), dist, seed)
             rng = np.random.default_rng(seed)
             x = rng.integers(-40, 41, size=(n, 33, 26)).astype(np.int8)
             x[:, :, 0] = rng.integers(1, 6, size=(n, 33))
@@ -216,7 +246,7 @@ def main():
                 srt = np.sort(want, 1)
                 clear = (srt[:, -1] - srt[:, -2]) > 1e-4
                 am = (p.numpy().argmax(1)[clear] != want.argmax(1)[clear]).sum()
-                print(f"variant seed {seed} {name:8s} max|dh| {eh:.2e}  max|dp| {ep:.2e}  argmax mismatches (clear) {am}", flush=True)
+                print(f"variant seed {seed} {dist} {name:8s} max|dh| {eh:.2e}  max|dp| {ep:.2e}  argmax mismatches (clear) {am}", flush=True)
     else:
         for seed in (4, 6):
             st = nets.make_polish_weights(seed)

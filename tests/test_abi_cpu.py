@@ -31,6 +31,13 @@ def test_every_declared_symbol_is_exported(lib):
     assert not missing, missing
 
 
+def test_q8_guard_threshold_matches_header():
+    src = open(os.path.join(ROOT, "include", "pepper_b200.h")).read()
+    m = re.search(r"#define\s+PB_VARIANT_Q8_MAX_GATE_ERR\s+(\S+)", src)
+    from pepper_b200 import abi
+    assert m and float(m.group(1)) == abi.PB_VARIANT_Q8_MAX_GATE_ERR
+
+
 def test_param_tables(lib):
     lib.pb_variant_net_param_name.restype = C.c_char_p
     lib.pb_variant_net_param_numel.restype = C.c_int64

@@ -38,13 +38,17 @@ def quantize(v):
     return np.rint(np.clip(v.astype(np.float32), -1, 1) * QS).astype(np.int64)
 
 
-@functools.lru_cache(maxsize=None)
-def weight_slices(d):
-    Wih, Whh, bias = lstm_params(1, d)
+def slices_of(Wih, Whh, bias):
     W = np.concatenate([Wih, Whh], axis=1)                         # torch row order; each row has its own scale
-    sw = 32512.0 / np.abs(W).max(axis=1)
+    m = np.abs(W).max(axis=1)
+    sw = 32512.0 / np.where(m > 0, m, 32512.0)                     # an all-zero row keeps sw = 1
     w1, w0 = qsplit(np.rint(W * sw[:, None]))
     return w1, w0, 1.0 / (32512.0 * sw), bias
+
+
+@functools.lru_cache(maxsize=None)
+def weight_slices(d):
+    return slices_of(*lstm_params(1, d))
 
 
 def untile_q(q, M, rows):
@@ -65,9 +69,9 @@ def variant_net_q8():
     return net
 
 
-def run_q8(M, persist, poison):
+def run_q8(M, persist, poison, net=None):
     from pepper_b200 import _lib
-    net = variant_net_q8()
+    net = net or variant_net_q8()
     x = np.ascontiguousarray(variant_inputs()[1][:M])
     mt = -(-M // 128)
     y = np.empty((M, VT, 512), np.float32)
@@ -78,9 +82,10 @@ def run_q8(M, persist, poison):
     return y, q, c
 
 
-def model_dir(x, d, fed1, fed0):
-    """x [R][33][512] fp32 input; fed1 / fed0 [R][33][256]: the kernel's h slices of direction d"""
-    w1, w0, inv, bias = weight_slices(d)
+def model_dir(x, d, fed1, fed0, slices=None):
+    """x [R][33][512] fp32 input; fed1 / fed0 [R][33][256]: the kernel's h slices of direction d; slices: slices_of() of
+    the direction's weights (default: variant_state()'s)"""
+    w1, w0, inv, bias = slices or weight_slices(d)
     a1, a0 = qsplit(quantize(x))
     R = x.shape[0]
     c = np.zeros((R, VH))

@@ -3,7 +3,7 @@ they are documented to perform.
 
 The model (no library code: it splits, scales and accumulates by itself):
   - every fp32 operand value v is split into fp16 hi = rn(clamp(v, +-65504)) and lo = rn(v - hi);
-  - each packed weight matrix W (an RNN direction: x-part and h-part together) is multiplied by s = 2^-ceil(log2 max|W|)
+  - each packed weight matrix W (an RNN direction: x-part and h-part together) is multiplied by s = 2^(15 - ceil(log2 max|W|))
     before the split, and the accumulator is multiplied by 1/s before the bias is added;
   - products: a_hi w_hi + a_hi w_lo, plus a_lo w_hi where that operand's lo flag is set, summed in float64;
   - cells with torch semantics (LSTM gates i, f, g, o; GRU r, z, n with n = tanh(W_in x + b_in + r (W_hn h + b_hn));
@@ -70,7 +70,7 @@ def split16(v):
 
 def pow2_scale(*mats):
     m = max(float(np.abs(w).max()) for w in mats)
-    return 2.0 ** -np.ceil(np.log2(m))
+    return 2.0 ** (15 - np.ceil(np.log2(m)))
 
 
 class SplitLinear:
@@ -289,8 +289,8 @@ def lstm_torch_fp32(layer):
     return y.numpy().astype(np.float64)
 
 
-def run_lstm(layer, M, lo_x, lo_h, persist, poison, tiles):
-    net = variant_net()
+def run_lstm(layer, M, lo_x, lo_h, persist, poison, tiles, net=None):
+    net = net or variant_net()
     x = np.ascontiguousarray(variant_inputs()[layer][:M])
     mt = -(-M // 128)
     y = np.empty((M, VT, 512), np.float32)
