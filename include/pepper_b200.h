@@ -397,8 +397,8 @@ int pb_variant_net_forward_host(pb_variant_net_t *net, const int8_t *h_images,
                                 int64_t n, float *h_probs, float *h_hidden_dbg,
                                 void *stream);
 /* GEMM path: 1 = wgmma with the fp16 hi/lo operand split (2-3 products per GEMM, see pb_variant_net_set_lo_mask), 2 = mode 1
- * with the decoder LSTM on int8 tensor cores; any other mode is PB_ERR_ARG.  pb_variant_net_create picks 2 when the decoder's
- * weights pass the int8 guard below, else 1; an explicit set_mode(2) is honoured either way.                                  */
+ * with the decoder LSTM and linear_1 on int8 tensor cores; any other mode is PB_ERR_ARG.  pb_variant_net_create picks 2 when
+ * the decoder's and linear_1's weights pass the int8 guards below, else 1; an explicit set_mode(2) is honoured either way.      */
 int pb_variant_net_set_mode(pb_variant_net_t *net, int mode);
 /* The int8 guard.  gate_err: the largest, over the decoder's gate rows, of a weight-only estimate of the error mode 2's 16-bit
  * weight slices (one scale per row, set by the row's largest |w|) and its dropped low x low product add to a gate
@@ -406,6 +406,12 @@ int pb_variant_net_set_mode(pb_variant_net_t *net, int mode);
  * below PB_VARIANT_Q8_MAX_GATE_ERR.  mode: the network's current mode.  Either pointer may be NULL.                           */
 #define PB_VARIANT_Q8_MAX_GATE_ERR 1e-4
 int pb_variant_net_q8_guard(pb_variant_net_t *net, double *gate_err, int *mode);
+/* The int8 guard of linear_1.  head_err: the largest, over linear_1's output rows, of a weight-only estimate of the error mode
+ * 2's weight slices (one scale per row), its dropped low x low product and the 16-bit fixed-point rounding of the decoder's h
+ * add to a pre-activation (DESIGN.md "linear_1 on int8 slices").  A network is created in mode 2 only when it is below
+ * PB_VARIANT_Q8_HEAD_MAX_ERR (and the decoder passes its guard).                                                             */
+#define PB_VARIANT_Q8_HEAD_MAX_ERR 3e-5
+int pb_variant_net_q8_head_err(pb_variant_net_t *net, double *head_err);
 int pb_variant_net_launches(pb_variant_net_t *net, int64_t *n_launches);
 
 /* ------------------------------------------------------------------------
@@ -465,6 +471,18 @@ int pb_test_variant_lstm_layer(pb_variant_net_t *net, int layer, int M, const vo
  * c_final [2][256][M].  poison: every buffer the launch touches starts as 0xff bytes. */
 int pb_test_variant_lstm_q8(pb_variant_net_t *net, int M, const float *h_x, int persist, int poison, float *h_y_f32, int8_t *h_q,
                             float *h_c_final);
+/* diagnostics: linear_1 of mode 2 (k_gemm_q8, the forward pass's own launch code) with the network's packed weights.  h_q: the
+ * decoder's h as int8 slices, int8 [2][M][33 * 512] (slice 1, then slice 0; feature t * 512 + d * 256 + unit).  Outputs (NULL =
+ * not written): h_out [M][512], SELU(h W^T + b) in fp32; h_y_hi / h_y_lo, the same as the fp16 operand tiles linear_2 reads
+ * [ceil(M / 128)][16][4096].  poison: output buffers start as NaN, padding rows of the slices as -1 bytes.                  */
+int pb_test_variant_head_q8(pb_variant_net_t *net, int M, const int8_t *h_q, int poison, float *h_out, uint16_t *h_y_hi,
+                            uint16_t *h_y_lo);
+/* diagnostics of the int8-slice weight packing (mode 2's decoder and linear_1): W fp32 [N][K], N % 128 == 0, K % 64 == 0 ->
+ * q = rint(sw_n W[n][k]) with sw_n = 32512 / max_k |W[n][k]| (1 for an all-zero row) as slices q = 256 w1 + w0, w1 =
+ * floor((q + 128) / 256), byte (n, k) at ((n / 128) * (K / 64) + k / 64) * 8192 + ((k % 64) / 16) * 2048 + (n % 128) * 16 + k % 16;
+ * col_scale[n] = 256 / (32512 sw_n); row_err[n], the guard's estimate for row n (a_quant: with the activation rounding term).
+ * No GPU needed.                                                                                                            */
+int pb_test_q8_pack(int N, int K, const float *h_W, int a_quant, int8_t *h_w1, int8_t *h_w0, float *h_col_scale, double *h_row_err);
 /* diagnostics: one bidirectional GRU layer (0 encoder, 1 decoder) of a polish network over one 100-step window on the wgmma
  * path.  h_x: uint8 [M][100][10] or fp32 [M][100][256]; h_h0: [2][M][128] or NULL (zero state).  Output: the sequence tiles
  * h_y_hi / h_y_lo [ceil(M / 128)][100][8][4096] (direction d of step t in k-tiles 8 t + 4 d .. 8 t + 4 d + 3).         */

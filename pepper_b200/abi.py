@@ -20,6 +20,8 @@ PB_ERR_STATE = -4
 
 # pb_variant_net_create runs the decoder in mode 2 only below this weight-only gate error estimate (pb_variant_net_q8_guard)
 PB_VARIANT_Q8_MAX_GATE_ERR = 1e-4
+# ... and linear_1 on int8 slices only below this one (pb_variant_net_q8_head_err)
+PB_VARIANT_Q8_HEAD_MAX_ERR = 3e-5
 
 
 class PbReads(C.Structure):

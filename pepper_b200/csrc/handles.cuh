@@ -9,16 +9,18 @@ struct VariantStream;      // streaming session state (pipeline.cu)
 // `scale`: the power of two s the tiles hold s W in (max |s W| in (2^14, 2^15]); the epilogues multiply by 1 / s
 struct TcRnn { DevBuf w_hi, w_lo, bias; int nkt_x = 0, nkt_h = 0; float scale = 1.f; };
 struct TcLin { DevBuf w_hi, w_lo, bias; int nkt = 0; float scale = 1.f; };
-// int8-slice decoder layer (mode 2, tc_gemm.cuh k_lstm_layer_q8): the two slices of round(sw_n W[n][k]), sw_n = 32512 /
-// max_k |W[n][k]| over K = [W_ih | W_hh], as [8 n-tiles][12 k-tiles][128][64] byte images, and the epilogue's
-// 256 / (32512 sw_n) per gate column n.  gate_err: the largest weight-only estimate over the rows of the error the slices add to
-// a gate pre-activation (nets_tc.cu tc_upload_rnn_q8); pb_variant_net_create compares it with PB_VARIANT_Q8_MAX_GATE_ERR
-struct TcRnnQ { DevBuf w1, w0, col_scale; double gate_err = 0.0; };
+// a weight matrix on int8 slices (mode 2: the decoder layer, tc_gemm.cuh k_lstm_layer_q8, and linear_1, k_gemm_q8): the two
+// slices of round(sw_n W[n][k]), sw_n = 32512 / max_k |W[n][k]| over the row's K (the decoder: [W_ih | W_hh]), as
+// [N / 128 n-tiles][K / 64 k-tiles][128][64] byte images, and the epilogue's 256 / (32512 sw_n) per output column n.  err: the
+// largest weight-only estimate over the rows of the error the slices add to a pre-activation (nets_tc.cu tc_upload_q8);
+// pb_variant_net_create compares it with PB_VARIANT_Q8_MAX_GATE_ERR (decoder) and PB_VARIANT_Q8_HEAD_MAX_ERR (linear_1)
+struct TcQ8 { DevBuf w1, w0, col_scale; double err = 0.0; };
 struct TcVariant {
     TcRnn enc[2], dec[2];
     TcLin lin[5];
-    TcRnnQ decq[2];
-    // mode 2: the encoder writes the decoder's x slices (q1 | q0) into yenc_lo, the decoder its own h slices into ydec_q
+    TcQ8 decq[2], lin1q;
+    // mode 2: the encoder writes the decoder's x slices (q1 | q0) into yenc_lo, the decoder its own h slices into ydec_q, and
+    // linear_1 reads those; ydec_hi / ydec_lo (the decoder's fp16 output) exist in mode 1 only
     DevBuf img_op, yenc_hi, yenc_lo, ydec_hi, ydec_lo, ydec_q, c, act_hi[2], act_lo[2], final_f32;
     // which GEMMs execute the third (a_lo x w_hi) product: bit 0 encoder h-part, 1 decoder x-part, 2 decoder h-part, 3 linear_1,
     // 4 linear_2..5; clearing a bit runs that GEMM with two products, 0x1f = three everywhere.  Default 0x1a: the recurrent
@@ -64,7 +66,8 @@ struct PolishStream;       // streaming polish session state (pipeline.cu)
 void polish_stream_free(PolishStream *S);
 int tc_upload_rnn(TcRnn &T, const float *Wp, const float *bias, int K0, int K0p_src, int H, int Kp_src);
 int tc_upload_lin(TcLin &T, const float *w, const float *bias, int N, int K);
-int tc_upload_rnn_q8(TcRnnQ &T, const float *Wp, int K0, int K0p_src, int H, int Kp_src);
+int tc_upload_rnn_q8(TcQ8 &T, const float *Wp, int K0, int K0p_src, int H, int Kp_src);
+int tc_upload_q8(TcQ8 &T, const float *W, int N, int K, bool a_quant);
 }  // namespace pb
 
 struct pb_variant_encoder {
@@ -117,10 +120,11 @@ struct pb_polish_encoder {
 
 struct pb_variant_net {
     int device = 0;
-    // 1 = wgmma GEMMs on the fp16 hi/lo operand split, 2 = mode 1 with the decoder LSTM on int8 tensor cores.
-    // pb_variant_net_create picks 2 when the decoder's weights pass the int8 guard (q8_gate_err < PB_VARIANT_Q8_MAX_GATE_ERR), else 1
+    // 1 = wgmma GEMMs on the fp16 hi/lo operand split, 2 = mode 1 with the decoder LSTM and linear_1 on int8 tensor cores.
+    // pb_variant_net_create picks 2 when both pass the int8 guard (q8_gate_err < PB_VARIANT_Q8_MAX_GATE_ERR and
+    // q8_head_err < PB_VARIANT_Q8_HEAD_MAX_ERR), else 1
     int mode = 2;
-    double q8_gate_err = 0.0;
+    double q8_gate_err = 0.0, q8_head_err = 0.0;
     pb::TcVariant tc;
     pb::DevBuf out_w, out_b;    // output_layer_type (3 x 512) for k_variant_out
     pb::DevBuf img, probs;      // host-entry staging

@@ -130,15 +130,18 @@ extern "C" int pb_variant_net_create(pb_variant_net_t **out, int device, const f
         PB_TRY(tc_upload_rnn(T.dec[d], pd.W.data(), pd.bias.data(), pd.K0, pd.K0p, VH, pd.Kp));
         PB_TRY(tc_upload_rnn_q8(T.decq[d], pd.W.data(), pd.K0, pd.K0p, VH, pd.Kp));
     }
+    // linear_1 twice: fp16 hi / lo tiles for mode 1, int8 slices for mode 2
     PB_TRY(tc_upload_lin(T.lin[0], P[16], P[17], 512, VT * 512));
+    PB_TRY(tc_upload_q8(T.lin1q, P[16], 512, VT * 512, true));
     for (int i = 1; i < 5; i++) PB_TRY(tc_upload_lin(T.lin[i], P[16 + 2 * i], P[17 + 2 * i], 512, 512));
     PB_TRY(upload(N->out_w, P[26], sizeof(float) * 3 * 512, 0));
     PB_TRY(upload(N->out_b, P[27], sizeof(float) * 3, 0));
-    // the int8 guard: weights whose slices would cost a gate more than the threshold run the decoder on the fp16 split instead,
-    // with all three products: the two-product recurrent GEMMs of mask 0x1a miss the parity gate on such weights too (an
-    // outlier of 100 std in W_hh multiplies the dropped a_lo, DESIGN.md "Int8-slice decoder")
-    N->q8_gate_err = std::max(T.decq[0].gate_err, T.decq[1].gate_err);
-    N->mode = N->q8_gate_err < PB_VARIANT_Q8_MAX_GATE_ERR ? 2 : 1;
+    // the int8 guard: weights whose slices would cost a gate or a linear_1 output more than its threshold run the network on
+    // the fp16 split instead, with all three products: the two-product recurrent GEMMs of mask 0x1a miss the parity gate on
+    // such weights too (an outlier of 100 std in W_hh multiplies the dropped a_lo, DESIGN.md "Int8-slice decoder")
+    N->q8_gate_err = std::max(T.decq[0].err, T.decq[1].err);
+    N->q8_head_err = T.lin1q.err;
+    N->mode = N->q8_gate_err < PB_VARIANT_Q8_MAX_GATE_ERR && N->q8_head_err < PB_VARIANT_Q8_HEAD_MAX_ERR ? 2 : 1;
     if (N->mode == 1) T.lo_mask = 0x1f;
     *out = N;
     return PB_OK;
@@ -151,6 +154,12 @@ extern "C" int pb_variant_net_q8_guard(pb_variant_net_t *N, double *gate_err, in
     return PB_OK;
 }
 
+extern "C" int pb_variant_net_q8_head_err(pb_variant_net_t *N, double *head_err) {
+    if (!N || !head_err) { set_error("null argument"); return PB_ERR_ARG; }
+    *head_err = N->q8_head_err;
+    return PB_OK;
+}
+
 extern "C" int pb_variant_net_destroy(pb_variant_net_t *N) {
     if (!N) return PB_OK;
     TcVariant &T = N->tc;
@@ -159,6 +168,7 @@ extern "C" int pb_variant_net_destroy(pb_variant_net_t *N) {
         for (auto *r : rnn) { r->w_hi.release(); r->w_lo.release(); r->bias.release(); }
         T.decq[d].w1.release(); T.decq[d].w0.release(); T.decq[d].col_scale.release();
     }
+    T.lin1q.w1.release(); T.lin1q.w0.release(); T.lin1q.col_scale.release();
     for (auto &l : T.lin) { l.w_hi.release(); l.w_lo.release(); l.bias.release(); }
     DevBuf *bufs[] = {&N->out_w, &N->out_b, &N->img, &N->probs, &T.img_op, &T.yenc_hi, &T.yenc_lo, &T.ydec_hi, &T.ydec_lo, &T.ydec_q,
                       &T.c, &T.act_hi[0], &T.act_hi[1], &T.act_lo[0], &T.act_lo[1], &T.final_f32};
@@ -170,7 +180,7 @@ extern "C" int pb_variant_net_destroy(pb_variant_net_t *N) {
 extern "C" int pb_variant_net_set_mode(pb_variant_net_t *N, int mode) {
     if (!N) return PB_ERR_ARG;
     if (mode != 1 && mode != 2) {
-        set_error("mode %d unknown (1 = tensor-core hi/lo x3, 2 = tensor cores with the int8-slice decoder LSTM)", mode);
+        set_error("mode %d unknown (1 = tensor-core hi/lo x3, 2 = tensor cores with the decoder LSTM and linear_1 on int8 slices)", mode);
         return PB_ERR_ARG;
     }
     N->mode = mode;

@@ -104,36 +104,47 @@ static inline int64_t qtiled_index(int64_t r, int64_t k, int64_t KT) {
     return ((r / 128) * KT + k / 64) * tc::QTILE_BYTES + ((k % 64) / 16) * 2048 + (r % 128) * 16 + (k % 16);
 }
 
-// the decoder direction's weights for k_lstm_layer_q8: rows 4j+g of Wp [4H][Kp_src] with K = [x | pad32 | h] -> K = [x | h].
-// T.gate_err: the largest over rows n of the weight-only error estimate of DESIGN.md "Int8-slice decoder" (guard),
-//   e_n = sqrt(sum_k (w_k / sw_n - W_k)^2 + (128^2 / 3) / 32512^2 sum_k (w0_k / sw_n)^2)
-// (weight rounding at |a_k| = 1, plus the dropped a0 w0 product with a0 uniform over its 8 bits).
-int tc_upload_rnn_q8(TcRnnQ &T, const float *Wp, int K0, int K0p_src, int H, int Kp_src) {
-    if (K0 % tc::QK || H % tc::QK || 4 * H % tc::QN) { set_error("int8 LSTM packing needs K0, H %% 64 == 0"); return PB_ERR_ARG; }
-    const int K = K0 + H, N = 4 * H, KT = K / tc::QK;
-    const double a0_var = 128.0 * 128.0 / 3.0 / ((double) tc::QSCALE * tc::QSCALE);
-    std::vector<int8_t> w1((size_t) N * K), w0((size_t) N * K);
-    std::vector<float> cs(N);
-    T.gate_err = 0.0;
+// W [N][K] row-major -> the slice images of TcQ8 (tiled with qtiled_index, K / 64 k-tiles per 128-row n-tile) and the column
+// scales.  row_err[n]: the weight-only estimate of the error the slices add to output n's pre-activation (DESIGN.md
+// "Int8-slice decoder" and "linear_1 on int8 slices"),
+//   e_n = sqrt(sum_k (w_k / sw_n - W_k)^2 + (128^2 / 3) / 32512^2 sum_k (w0_k / sw_n)^2 [+ sum_k W_k^2 / (12 32512^2)])
+// (weight rounding at |a_k| = 1, plus the dropped a0 w0 product with a0 uniform over its 8 bits; a_quant adds the rounding of
+// fp32 activations to 1 / 32512 steps, which linear_1's fp16 path does not have).
+static void pack_q8(const float *W, int N, int K, bool a_quant, std::vector<int8_t> &w1, std::vector<int8_t> &w0,
+                    std::vector<float> &cs, std::vector<double> &row_err) {
+    const int KT = K / tc::QK;
+    const double qs2 = (double) tc::QSCALE * tc::QSCALE;
+    const double a0_var = 128.0 * 128.0 / 3.0 / qs2;
+    w1.assign((size_t) N * K, 0); w0.assign((size_t) N * K, 0);
+    cs.assign(N, 0.f); row_err.assign(N, 0.0);
     for (int n = 0; n < N; n++) {
-        const float *x = Wp + (size_t) n * Kp_src, *h = x + K0p_src;
+        const float *x = W + (size_t) n * K;
         double m = 0.0;
-        for (int k = 0; k < K0; k++) m = std::max(m, (double) std::fabs(x[k]));
-        for (int k = 0; k < H; k++) m = std::max(m, (double) std::fabs(h[k]));
+        for (int k = 0; k < K; k++) m = std::max(m, (double) std::fabs(x[k]));
         const double sw = m > 0.0 && std::isfinite(m) ? tc::QSCALE / m : 1.0;
         cs[n] = (float) (256.0 / (tc::QSCALE * sw));
-        double e_round = 0.0, e_drop = 0.0;
+        double e_round = 0.0, e_drop = 0.0, sq = 0.0;
         for (int k = 0; k < K; k++) {
             const int64_t o = qtiled_index(n, k, KT);
-            const double w = k < K0 ? x[k] : h[k - K0];
+            const double w = x[k];
             int8_t &s1 = w1[(size_t) o], &s0 = w0[(size_t) o];
             qsplit(w * sw, s1, s0);
             const double r = (256.0 * s1 + s0) / sw - w, d = s0 / sw;
             e_round += r * r;
             e_drop += d * d;
+            sq += w * w;
         }
-        T.gate_err = std::max(T.gate_err, std::sqrt(e_round + a0_var * e_drop));
+        row_err[n] = std::sqrt(e_round + a0_var * e_drop + (a_quant ? sq / (12.0 * qs2) : 0.0));
     }
+}
+
+int tc_upload_q8(TcQ8 &T, const float *W, int N, int K, bool a_quant) {
+    if (K % tc::QK || N % tc::QN) { set_error("int8 slice packing needs N %% 128 == 0 and K %% 64 == 0"); return PB_ERR_ARG; }
+    std::vector<int8_t> w1, w0;
+    std::vector<float> cs;
+    std::vector<double> err;
+    pack_q8(W, N, K, a_quant, w1, w0, cs, err);
+    T.err = *std::max_element(err.begin(), err.end());
     PB_TRY(T.w1.reserve(w1.size()));
     PB_TRY(T.w0.reserve(w0.size()));
     PB_TRY(T.col_scale.reserve(sizeof(float) * N));
@@ -141,6 +152,16 @@ int tc_upload_rnn_q8(TcRnnQ &T, const float *Wp, int K0, int K0p_src, int H, int
     PB_CUDA(cudaMemcpy(T.w0.p, w0.data(), w0.size(), cudaMemcpyHostToDevice));
     PB_CUDA(cudaMemcpy(T.col_scale.p, cs.data(), sizeof(float) * N, cudaMemcpyHostToDevice));
     return PB_OK;
+}
+// the decoder direction's weights for k_lstm_layer_q8: rows 4j+g of Wp [4H][Kp_src] with K = [x | pad32 | h] -> K = [x | h]
+int tc_upload_rnn_q8(TcQ8 &T, const float *Wp, int K0, int K0p_src, int H, int Kp_src) {
+    const int K = K0 + H, N = 4 * H;
+    std::vector<float> W((size_t) N * K);
+    for (int n = 0; n < N; n++) {
+        std::copy(Wp + (size_t) n * Kp_src, Wp + (size_t) n * Kp_src + K0, W.begin() + (size_t) n * K);
+        std::copy(Wp + (size_t) n * Kp_src + K0p_src, Wp + (size_t) n * Kp_src + K0p_src + H, W.begin() + (size_t) n * K + K0);
+    }
+    return tc_upload_q8(T, W.data(), N, K, false);
 }
 
 static int g_num_sms = 0;
@@ -278,8 +299,8 @@ static int variant_lstm_layer_tc(pb_variant_net *N, int layer, int64_t B, bool l
     return PB_OK;
 }
 
-// The int8-slice decoder layer (mode 2): x = the encoder's slices in T.yenc_lo, h slices in T.ydec_q, fp16 hi / lo output
-// tiles in T.ydec_hi / T.ydec_lo for linear_1 (+ the optional fp32 copy).  persist: one k_lstm_layer_q8 launch for all 33
+// The int8-slice decoder layer (mode 2): x = the encoder's slices in T.yenc_lo, h slices in T.ydec_q (its own h-part and
+// linear_1's A operand) (+ the optional fp32 copy).  persist: one k_lstm_layer_q8 launch for all 33
 // steps (the forward pass), or one launch per step, the reference for the in-kernel h hand-off (pb_test_variant_lstm_q8).
 static int variant_dec_q8(pb_variant_net *N, int64_t B, bool persist, float *y_f32, cudaStream_t st) {
     TcVariant &T = N->tc;
@@ -296,7 +317,6 @@ static int variant_dec_q8(pb_variant_net *N, int64_t B, bool persist, float *y_f
         L.col_scale[d] = T.decq[d].col_scale.as<float>();
         L.c[d] = T.c.as<float>() + (int64_t) d * VH * Bp;
     }
-    L.y_hi = T.ydec_hi.as<bf16>(); L.y_lo = T.ydec_lo.as<bf16>(); L.y_mt_stride = (int64_t) VT * 16 * TILE_ELEMS;
     if (y_f32) { L.y_f32 = y_f32; L.ldy = (int64_t) VT * 512; }
     L.M = (int) B; L.n_mt = (int) Mt; L.T = VT; L.c_ld = Bp;
     static bool attr_set = false;
@@ -312,15 +332,46 @@ static int variant_dec_q8(pb_variant_net *N, int64_t B, bool persist, float *y_f
     return PB_OK;
 }
 
-// scratch of one chunk of B candidates
-static int variant_reserve_tc(TcVariant &T, int64_t B) {
+// linear_1 on int8 slices (mode 2): SELU(ydec W^T + b) from the decoder's h slices in T.ydec_q, all 33 steps read in place
+// (slice k-tile tt * 8 + dir * 4 + unit / 64 is feature tt * 512 + dir * 256 + unit, linear_1's K order), into the fp16 tiles
+// T.act_hi[0] / T.act_lo[0] that linear_2 reads (+ the optional fp32 copy y_f32 [B][512]).  One k_gemm_q8 launch.
+static int variant_lin1_q8(pb_variant_net *N, int64_t B, float *y_f32, cudaStream_t st) {
+    TcVariant &T = N->tc;
+    const int64_t Mt = ceil_div(B, 128);
+    tc::GemmQ G;
+    memset(&G, 0, sizeof(G));
+    G.a1 = T.ydec_q.as<int8_t>(); G.a0 = G.a1 + Mt * q_mt_bytes(); G.a_mt_stride = q_mt_bytes();
+    G.w1 = T.lin1q.w1.as<int8_t>(); G.w0 = T.lin1q.w0.as<int8_t>();
+    G.bias = T.lin[0].bias.as<float>(); G.col_scale = T.lin1q.col_scale.as<float>();
+    G.y_hi = T.act_hi[0].as<bf16>(); G.y_lo = T.act_lo[0].as<bf16>(); G.y_f32 = y_f32;
+    G.M = (int) B; G.N = 512; G.n_mt = (int) Mt; G.nkt = VT * 8;
+    static bool attr_set = false;
+    if (!attr_set) {
+        PB_CUDA(cudaFuncSetAttribute(tc::k_gemm_q8, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::GQSMEM_BYTES));
+        attr_set = true;
+    }
+    if (g_num_sms == 0) {
+        int dev = 0;
+        PB_CUDA(cudaGetDevice(&dev));
+        PB_CUDA(cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev));
+    }
+    const int tiles = (int) Mt * (G.N / tc::QN);
+    tc::k_gemm_q8<<<(unsigned) std::min(tiles, g_num_sms), tc::PG_THREADS, tc::GQSMEM_BYTES, st>>>(G);
+    N->launches++;
+    return PB_OK;
+}
+
+// scratch of one chunk of B candidates; the decoder's fp16 output tiles only for mode 1 (mode 2's linear_1 reads the slices)
+static int variant_reserve_tc(TcVariant &T, int64_t B, int mode) {
     const int64_t Mt = ceil_div(B, 128), Bp = Mt * 128;
     const int64_t seq_tiles = Mt * VT * 16;                 // [mt][t][16 k-tiles] of a 512-feature sequence operand
     PB_TRY(T.img_op.reserve((size_t) (Mt * VT * TILE_ELEMS) * 2));
     PB_TRY(T.yenc_hi.reserve((size_t) (seq_tiles * TILE_ELEMS) * 2));
     PB_TRY(T.yenc_lo.reserve((size_t) (seq_tiles * TILE_ELEMS) * 2));
-    PB_TRY(T.ydec_hi.reserve((size_t) (seq_tiles * TILE_ELEMS) * 2));
-    PB_TRY(T.ydec_lo.reserve((size_t) (seq_tiles * TILE_ELEMS) * 2));
+    if (mode == 1) {
+        PB_TRY(T.ydec_hi.reserve((size_t) (seq_tiles * TILE_ELEMS) * 2));
+        PB_TRY(T.ydec_lo.reserve((size_t) (seq_tiles * TILE_ELEMS) * 2));
+    }
     PB_TRY(T.ydec_q.reserve((size_t) (2 * Mt * q_mt_bytes())));
     PB_TRY(T.c.reserve(sizeof(float) * 2 * VH * Bp));
     for (int i = 0; i < 2; i++) {
@@ -372,7 +423,7 @@ int variant_forward_tc(pb_variant_net *N, const int8_t *d_images, int64_t B, flo
                        const OutSink &sink) {
     TcVariant &T = N->tc;
     const int64_t Mt = ceil_div(B, 128), Bp = Mt * 128;
-    PB_TRY(variant_reserve_tc(T, B));
+    PB_TRY(variant_reserve_tc(T, B, N->mode));
 
     tc::k_tc_pack_images<<<(unsigned) ceil_div(Bp * VT * 4, 256), 256, 0, st>>>(d_images, T.img_op.as<bf16>(), B, VT, 26);
     N->launches++;
@@ -388,6 +439,10 @@ int variant_forward_tc(pb_variant_net *N, const int8_t *d_images, int64_t B, flo
     }
     // MLP head
     for (int i = 0; i < 5; i++) {
+        if (i == 0 && N->mode == 2) {
+            PB_TRY(variant_lin1_q8(N, B, nullptr, st));
+            continue;
+        }
         Args A;
         A.M = (int) B; A.N = 512; A.c_ld = 0;
         Dir D = empty_dir();
@@ -690,7 +745,7 @@ extern "C" int pb_test_variant_lstm_layer(pb_variant_net_t *net, int layer, int 
     PB_CUDA(cudaSetDevice(net->device));
     TcVariant &T = net->tc;
     const int64_t Mt = ceil_div(M, 128), Bp = Mt * 128, seq = Mt * VT * 16 * TILE_ELEMS;
-    PB_TRY(variant_reserve_tc(T, M));
+    PB_TRY(variant_reserve_tc(T, M, 1));
     if (poison) {
         DevBuf *bufs[] = {&T.img_op, &T.yenc_hi, &T.yenc_lo, &T.ydec_hi, &T.ydec_lo, &T.c};
         for (auto *b : bufs) PB_TRY(fill_nan(*b));
@@ -733,9 +788,9 @@ extern "C" int pb_test_variant_lstm_q8(pb_variant_net_t *net, int M, const float
     PB_CUDA(cudaSetDevice(net->device));
     TcVariant &T = net->tc;
     const int64_t Mt = ceil_div(M, 128), Bp = Mt * 128, qbytes = Mt * q_mt_bytes();
-    PB_TRY(variant_reserve_tc(T, M));
+    PB_TRY(variant_reserve_tc(T, M, 2));
     if (poison) {
-        DevBuf *bufs[] = {&T.yenc_lo, &T.ydec_hi, &T.ydec_lo, &T.ydec_q, &T.c};
+        DevBuf *bufs[] = {&T.yenc_lo, &T.ydec_q, &T.c};
         for (auto *b : bufs) PB_TRY(fill_nan(*b));
     }
     // the encoder's quantization (tc_gemm.cuh qsplit2): rint(fp32(clamp(x, -1, 1) * 32512))
@@ -761,6 +816,57 @@ extern "C" int pb_test_variant_lstm_q8(pb_variant_net_t *net, int M, const float
         for (int d = 0; d < 2; d++)
             PB_CUDA(cudaMemcpy2D(h_c_final + (size_t) d * VH * M, sizeof(float) * M, T.c.as<float>() + (int64_t) d * VH * Bp,
                                  sizeof(float) * Bp, sizeof(float) * M, VH, cudaMemcpyDeviceToHost));
+    return PB_OK;
+}
+
+// linear_1 of mode 2 (variant_lin1_q8, the forward pass's own launch code) on host-given slices of the decoder's h.
+extern "C" int pb_test_variant_head_q8(pb_variant_net_t *net, int M, const int8_t *h_q, int poison, float *h_out, uint16_t *h_y_hi,
+                                       uint16_t *h_y_lo) {
+    if (!net || M <= 0 || !h_q || (!h_y_hi) != (!h_y_lo)) { set_error("pb_test_variant_head_q8: bad argument"); return PB_ERR_ARG; }
+    PB_CUDA(cudaSetDevice(net->device));
+    TcVariant &T = net->tc;
+    const int64_t Mt = ceil_div(M, 128), qbytes = Mt * q_mt_bytes(), K = VT * 512, act = Mt * 16 * TILE_ELEMS;
+    PB_TRY(variant_reserve_tc(T, M, 2));
+    if (poison) {
+        DevBuf *bufs[] = {&T.act_hi[0], &T.act_lo[0]};
+        for (auto *b : bufs) PB_TRY(fill_nan(*b));
+    }
+    std::vector<int8_t> q(2 * qbytes, poison ? (int8_t) -1 : (int8_t) 0);
+    for (int s = 0; s < 2; s++)
+        for (int64_t r = 0; r < M; r++)
+            for (int64_t k = 0; k < K; k++) q[s * qbytes + qtiled_index(r, k, VT * 8)] = h_q[(s * (int64_t) M + r) * K + k];
+    PB_CUDA(cudaMemcpy(T.ydec_q.p, q.data(), q.size(), cudaMemcpyHostToDevice));
+    Scratch S;
+    if (h_out) {
+        PB_TRY(S.b[0].reserve(sizeof(float) * (size_t) M * 512));
+        PB_CUDA(cudaMemset(S.b[0].p, poison ? 0xff : 0, S.b[0].cap));
+    }
+    PB_TRY(variant_lin1_q8(net, M, h_out ? S.b[0].as<float>() : nullptr, 0));
+    PB_CUDA(cudaGetLastError());
+    PB_CUDA(cudaDeviceSynchronize());
+    if (h_out) PB_CUDA(cudaMemcpy(h_out, S.b[0].p, sizeof(float) * (size_t) M * 512, cudaMemcpyDeviceToHost));
+    if (h_y_hi) {
+        PB_CUDA(cudaMemcpy(h_y_hi, T.act_hi[0].p, (size_t) act * 2, cudaMemcpyDeviceToHost));
+        PB_CUDA(cudaMemcpy(h_y_lo, T.act_lo[0].p, (size_t) act * 2, cudaMemcpyDeviceToHost));
+    }
+    return PB_OK;
+}
+
+// The host packing of a weight matrix on int8 slices (pack_q8).  No GPU needed.
+extern "C" int pb_test_q8_pack(int N, int K, const float *h_W, int a_quant, int8_t *h_w1, int8_t *h_w0, float *h_col_scale,
+                               double *h_row_err) {
+    if (N <= 0 || K <= 0 || N % tc::QN || K % tc::QK || !h_W || !h_w1 || !h_w0 || !h_col_scale || !h_row_err) {
+        set_error("pb_test_q8_pack: N %% 128 and K %% 64 must be 0");
+        return PB_ERR_ARG;
+    }
+    std::vector<int8_t> w1, w0;
+    std::vector<float> cs;
+    std::vector<double> err;
+    pack_q8(h_W, N, K, a_quant != 0, w1, w0, cs, err);
+    memcpy(h_w1, w1.data(), w1.size());
+    memcpy(h_w0, w0.data(), w0.size());
+    memcpy(h_col_scale, cs.data(), sizeof(float) * N);
+    memcpy(h_row_err, err.data(), sizeof(double) * N);
     return PB_OK;
 }
 

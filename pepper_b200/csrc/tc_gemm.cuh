@@ -151,7 +151,7 @@ __device__ __forceinline__ void wgmma_256(float (&d)[128], uint64_t adesc, uint6
         : "l"(adesc), "l"(bdesc), "r"(1));
 }
 
-// ---------------------------------------------------------------- int8-slice operands (decoder LSTM layer, mode 2)
+// ---------------------------------------------------------------- int8-slice operands (mode 2: decoder LSTM layer and linear_1)
 // A value v in [-1, 1] (an LSTM hidden state) is held as the 16-bit fixed-point integer q = rint(v * 32512) split into two
 // signed int8 slices, q = 256 q1 + q0 with q1 = floor((q + 128) / 256) in [-127, 127] and q0 in [-128, 127].  A weight row
 // (gate column n, K = [W_ih | W_hh]) is held the same way at its own scale sw_n = 32512 / max_k |W[n][k]|.  Three s8 x s8
@@ -168,6 +168,7 @@ constexpr int QN = 128;                             // gate columns per tile (32
 constexpr int QSTAGES = 6;
 constexpr int QSTAGE_BYTES = 4 * QTILE_BYTES;       // a1, a0, w1, w0 = 32 KB
 constexpr int QSMEM_BYTES = QSTAGES * QSTAGE_BYTES + 256 + 2 * 1024 * 4;   // ring + barriers + bias + column scales
+constexpr int GQSMEM_BYTES = QSTAGES * QSTAGE_BYTES + 256;                  // k_gemm_q8: ring + barriers
 constexpr float QSCALE = 32512.f;
 
 // d[64 x 128] (s32) += A[64 x 32] B[128 x 32]^T, s8 operands K-major in shared memory
@@ -625,9 +626,9 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
 // k_lstm_layer's structure (one CTA per (direction, row tile) for all steps, one producer thread streaming whole tiles onto an
 // mbarrier ring, h_t handed to the producer through bar_h) with int8-slice operands: K = [x (512) | h (256)] = 12 k-tiles of
 // 64, 128-column gate tiles (32 units x 4 gates, 8 per step) so that the two int32 accumulators of a warpgroup take the 128
-// registers one fp32 accumulator took.  Each step writes h_t as fp16 hi / lo operand tiles (linear_1) and as int8 slices (its
-// own h-part of the next step).  Steps t0 .. t1 - 1 run in one launch: the cell state and h stay in HBM between launches, so
-// one launch per step is the cross-check of the in-kernel hand-off.
+// registers one fp32 accumulator took.  Each step writes h_t only as int8 slices: they are the h-part of its own next step and,
+// all 33 steps together, the A operand of linear_1 (k_gemm_q8).  Steps t0 .. t1 - 1 run in one launch: the cell state and h
+// stay in HBM between launches, so one launch per step is the cross-check of the in-kernel hand-off.
 struct LstmLayerQ {
     const int8_t *x1, *x0;             // input sequence slices (QSeq): tile (mt, tt, kt) at mt * q_mt_stride + (tt * 8 + kt) * QTILE_BYTES
     const int8_t *w1[2], *w0[2];       // per direction: [8 n-tiles][12 k-tiles][QTILE_BYTES]
@@ -636,8 +637,6 @@ struct LstmLayerQ {
     float *c[2];                       // cell state per direction [256][c_ld]
     int8_t *q1, *q0;                   // output sequence slices (QSeq); direction d -> k-tiles 4 d .. 4 d + 3
     int64_t q_mt_stride;               // bytes, the same for x and q
-    op_t *y_hi, *y_lo;                 // output sequence operand [mt][T][16] fp16 tiles
-    int64_t y_mt_stride;
     float *y_f32;                      // optional fp32 copy [row][T][512]
     int64_t ldy;
     int M, n_mt, T, t0, t1;
@@ -751,15 +750,13 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer_q8(LstmLayerQ G)
             int c2s;
             asm volatile("mov.b32 %0, %1;" : "=r"(c2s) : "r"(c2));
             const float *sb = sbias + nt * QN + 2 * q, *ss = sscale + nt * QN + 2 * q;
-            // units nt * 32 .. + 31: fp16 k-tile dir * 8 + nt, slice k-tile 4 dir + nt / 2 (chunks 2 (nt & 1), + 1).  The
-            // even-unit lane writes the hi words and slice 1 of a unit pair, the odd-unit lane the lo words and slice 0.
-            op_t *yw = (odd_u ? G.y_lo : G.y_hi) + (int64_t) mt * G.y_mt_stride + (int64_t) (tt * 16 + dir * 8 + nt) * TILE_ELEMS + r128 * 8;
+            // units nt * 32 .. + 31: slice k-tile 4 dir + nt / 2 (chunks 2 (nt & 1), + 1).  The even-unit lane writes slice 1
+            // of a unit pair, the odd-unit lane slice 0.
             int8_t *qw = (odd_u ? G.q0 : G.q1) + mt * G.q_mt_stride + (int64_t) (tt * 8 + dir * 4 + (nt >> 1)) * QTILE_BYTES +
                          (nt & 1) * 2 * 2048 + r128 * 16;
             float *yf = G.y_f32 ? G.y_f32 + (int64_t) row * G.ldy + (int64_t) tt * 512 + dir * 256 + nt * (QN / 4) : nullptr;
 #pragma unroll
             for (int m = 0; m < QN / 16; m++) {
-                uint32_t w[2];
                 int uq[4];
 #pragma unroll
                 for (int e = 0; e < 2; e++) {
@@ -779,14 +776,10 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer_q8(LstmLayerQ G)
                     if (valid) cp[i * c2s] = cn;
                     const float hp = __shfl_xor_sync(0xffffffffu, hn, 2);
                     const float h0 = odd_u ? hp : hn, h1 = odd_u ? hn : hp;          // units 2 i, 2 i + 1
-                    uint32_t hi, lo;
-                    split2<true>(h0, h1, hi, lo);
-                    w[e] = odd_u ? lo : hi;
                     uq[2 * e] = qbias(h0); uq[2 * e + 1] = qbias(h1);
                     if (yf && valid && !odd_u) *reinterpret_cast<float2 *>(yf + 2 * i) = make_float2(h0, h1);
                 }
                 // units nt * 32 + 4 m .. + 3 of row r128
-                if (valid) __stwb(reinterpret_cast<uint2 *>(yw + (m >> 1) * 1024 + 4 * (m & 1)), make_uint2(w[0], w[1]));
                 if (valid) __stwb(reinterpret_cast<uint32_t *>(qw + (m >> 2) * 2048 + 4 * (m & 3)), qword(uq[0], uq[1], uq[2], uq[3], odd_u));
             }
         }
@@ -794,6 +787,107 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer_q8(LstmLayerQ G)
         __threadfence();
         __syncwarp();
         if (lane == 0) mbar_arrive(bar_h);
+    }
+}
+
+// ---------------------------------------------------------------- persistent GEMM on int8 slices (linear_1, mode 2)
+// Y = SELU(A W^T + bias) with A in [-1, 1] held as QSeq slices (the decoder's h, all 33 steps, read in place) and W packed per
+// output row like the decoder's gate rows.  k_tc_gemm_p's tile loop (one CTA per SM, static round-robin over 128 x 128
+// output tiles, nt fastest so that CTAs running together share the A row tile) around k_lstm_layer_q8's k-loop: the
+// producer thread streams a1, a0, w1, w0 of one 64-k tile per ring stage and runs ahead across tiles, so the next tile's
+// operands arrive while the consumers apply the epilogue of the current one.  No split-K: a row's outputs do not depend on
+// which other rows share its launch.  |acc_hh| <= K 127^2 and |acc_mix| <= 2 K 127 128 stay below 2^31 for K < 65,000.
+struct GemmQ {
+    const int8_t *a1, *a0;             // A slices: tile (mt, kt) at mt * a_mt_stride + kt * QTILE_BYTES
+    int64_t a_mt_stride;               // bytes
+    const int8_t *w1, *w0;             // [N / 128 n-tiles][nkt][QTILE_BYTES]
+    const float *bias, *col_scale;     // [N]; col_scale 256 / (32512 sw_n)
+    op_t *y_hi, *y_lo;                 // output operand tiles [mt][N / 32][TILE_ELEMS] (the next layer's A)
+    float *y_f32;                      // optional fp32 copy [M][N]
+    int M, N, n_mt, nkt;
+};
+
+__global__ void __launch_bounds__(PG_THREADS, 1) k_gemm_q8(GemmQ G) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + QSTAGES * QSTAGE_BYTES);
+    const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + QSTAGES);
+    const uint32_t smem_base = smem_u32(smem);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int n_nt = G.N / QN, n_tiles = G.n_mt * n_nt;
+
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < QSTAGES; s++) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, CONS_WARPS); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    if (warp == CONS_WARPS) {
+        if (lane == 0) {
+            uint32_t g = 0;                                   // running k-tile counter across tiles
+            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+                const int nt = tile % n_nt, mt = tile / n_nt;
+                const int64_t aoff = (int64_t) mt * G.a_mt_stride, woff = (int64_t) nt * G.nkt * QTILE_BYTES;
+                for (int kt = 0; kt < G.nkt; kt++, g++) {
+                    const int64_t ko = (int64_t) kt * QTILE_BYTES;
+                    load_stage_q(smem_base, bar_full, bar_empty, g, G.a1 + aoff + ko, G.a0 + aoff + ko, G.w1 + woff + ko, G.w0 + woff + ko);
+                }
+            }
+        }
+        return;
+    }
+    const int wg = warp >> 2, q = lane & 3;
+    const int rA = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    uint32_t g = 0;
+    int hh[64], mix[64];
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const int nt = tile % n_nt, mt = tile / n_nt;
+#pragma unroll
+        for (int i = 0; i < 64; i++) { hh[i] = 0; mix[i] = 0; }
+        for (int kt = 0; kt < G.nkt; kt++, g++) {
+            const uint32_t s = g % QSTAGES, ph = (g / QSTAGES) & 1u;
+            mbar_wait(bar_full + 8 * s, ph);
+            const uint32_t st = smem_base + s * QSTAGE_BYTES, a = st + (uint32_t) wg * 1024, b = st + 2 * QTILE_BYTES;
+            wg_fence();
+#pragma unroll
+            for (int ks = 0; ks < QK / 32; ks++) {
+                const uint64_t a1 = smem_desc(a + ks * 4096, 2048), a0 = smem_desc(a + QTILE_BYTES + ks * 4096, 2048);
+                const uint64_t w1 = smem_desc(b + ks * 4096, 2048), w0 = smem_desc(b + QTILE_BYTES + ks * 4096, 2048);
+                wgmma_q8(hh, a1, w1);
+                wgmma_q8(mix, a1, w0);
+                wgmma_q8(mix, a0, w1);
+            }
+            wg_commit();
+            wg_wait<1>();
+            if (kt > 0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(bar_empty + 8 * ((g - 1) % QSTAGES));
+            }
+        }
+        wg_wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_empty + 8 * ((g - 1) % QSTAGES));
+        // accumulator fragment of m64n128: [4 i + e] is row rA + 8 (e >> 1), column 8 i + 2 q + (e & 1)
+#pragma unroll
+        for (int i = 0; i < QN / 8; i++) {
+            const int col = nt * QN + 8 * i + 2 * q;
+            const float2 bz = __ldg(reinterpret_cast<const float2 *>(G.bias + col));
+            const float2 sz = __ldg(reinterpret_cast<const float2 *>(G.col_scale + col));
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                const int r128 = rA + 8 * h, row = mt * BM + r128;
+                const int e = 4 * i + 2 * h;
+                const float v0 = selu(fmaf(fmaf((float) hh[e], 256.f, (float) mix[e]), sz.x, bz.x));
+                const float v1 = selu(fmaf(fmaf((float) hh[e + 1], 256.f, (float) mix[e + 1]), sz.y, bz.y));
+                if (row < G.M) {
+                    uint32_t hi, lo;
+                    split2(v0, v1, hi, lo);
+                    const int64_t o = (int64_t) mt * (G.N / BK) * TILE_ELEMS + tile_off(col, r128);
+                    *reinterpret_cast<uint32_t *>(G.y_hi + o) = hi;
+                    *reinterpret_cast<uint32_t *>(G.y_lo + o) = lo;
+                    if (G.y_f32) *reinterpret_cast<float2 *>(G.y_f32 + (int64_t) row * G.N + col) = make_float2(v0, v1);
+                }
+            }
+        }
     }
 }
 

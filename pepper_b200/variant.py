@@ -190,9 +190,10 @@ class VariantNet:
 
     def set_mode(self, mode: int) -> None:
         """1 = wgmma GEMMs with the 16-bit hi/lo operand split (2-3 products per GEMM, set_lo_mask), 2 = mode 1 with the
-        decoder LSTM on int8 tensor cores: 16-bit fixed-point operands as two int8 slices, exact int32 accumulation
-        (DESIGN.md section 4); any other mode raises PepperB200Error.  A new network is in mode 2 when its decoder weights
-        pass the int8 guard (`q8_gate_err`), else in mode 1; setting a mode here overrides that choice."""
+        decoder LSTM and linear_1 on int8 tensor cores: 16-bit fixed-point operands as two int8 slices, exact int32
+        accumulation (DESIGN.md section 4); any other mode raises PepperB200Error.  A new network is in mode 2 when its
+        decoder and linear_1 weights pass the int8 guards (`q8_gate_err`, `head_q8_err`), else in mode 1; setting a mode
+        here overrides that choice."""
         _lib.check(self.L.pb_variant_net_set_mode(self.h, mode), "pb_variant_net_set_mode")
 
     def _q8_guard(self) -> tuple[float, int]:
@@ -211,6 +212,15 @@ class VariantNet:
         """weight-only estimate of the error the int8 decoder adds to a gate pre-activation (largest over gate rows); the
         network was created in mode 2 only if it is below abi.PB_VARIANT_Q8_MAX_GATE_ERR"""
         return self._q8_guard()[0]
+
+    @property
+    def head_q8_err(self) -> float:
+        """weight-only estimate of the error int8 linear_1 adds to a pre-activation (largest over output rows); the network
+        was created in mode 2 only if it is below abi.PB_VARIANT_Q8_HEAD_MAX_ERR (and q8_gate_err below its threshold)"""
+        err = C.c_double(0.0)
+        self.L.pb_variant_net_q8_head_err.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
+        _lib.check(self.L.pb_variant_net_q8_head_err(self.h, C.byref(err)), "pb_variant_net_q8_head_err")
+        return float(err.value)
 
     def set_lo_mask(self, mask: int) -> None:
         """Bit set = that GEMM keeps its third tensor-core product (a_lo x w_hi).  bits: 0 encoder h-part, 1 decoder x-part,

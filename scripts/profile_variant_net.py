@@ -7,7 +7,9 @@ every CTA streams.
 
     python scripts/profile_variant_net.py [--sizes 8448 1408] [--reps 5] [--mode 2] [--out FILE]     (PB_LIB_PATH selects the build)
 
-In mode 2 the decoder layer is k_lstm_layer_q8 (int8 slices); --mode 1 profiles the fp16 hi/lo decoder of the same build.
+In mode 2 the decoder layer is k_lstm_layer_q8 and linear_1 is k_gemm_q8 (int8 slices); --mode 1 profiles the fp16 hi/lo
+decoder and linear_1 of the same build.  The first head launch of each predict is reported as linear_1, the other four as
+head_gemm (linear_2 .. linear_5).
 """
 import argparse
 import json
@@ -22,7 +24,7 @@ sys.path.insert(0, ROOT)
 
 
 def label(name: str) -> str:
-    for key, short in (("k_lstm_layer", "lstm_layer"), ("k_tc_gemm_p", "head_gemm"), ("k_tc_pack_images", "pack_images"),
+    for key, short in (("k_lstm_layer", "lstm_layer"), ("k_tc_gemm_p", "head_gemm"), ("k_gemm_q8", "head_gemm"), ("k_tc_pack_images", "pack_images"),
                        ("k_variant_out", "out_softmax")):
         if key in name:
             return short
@@ -51,12 +53,16 @@ def profile_size(net, n: int, reps: int, rng) -> dict:
     kernels = sorted((e for e in prof.events() if e.device_type == DeviceType.CUDA and "memcpy" not in e.name.lower()
                       and "memset" not in e.name.lower()), key=lambda e: e.time_range.start)
     per = {}
-    n_lstm = 0
+    n_lstm = n_head = 0
     for e in kernels:
         k = label(e.name)
         if k == "lstm_layer":                       # two launches per predict: encoder, then decoder
             k = ("encoder_" if n_lstm % 2 == 0 else "decoder_") + k
             n_lstm += 1
+        elif k == "head_gemm":                      # five launches per chunk: linear_1, then linear_2 .. linear_5
+            if n_head % 5 == 0:
+                k = "linear_1"
+            n_head += 1
         per.setdefault(k, []).append(e.time_range.elapsed_us() / 1e3)
     ms = {k: {"ms_per_predict": sum(v) / reps, "launches_per_predict": len(v) / reps} for k, v in per.items()}
     sm = [float(r) for r in rows if r.replace(".", "", 1).isdigit()]

@@ -11,7 +11,11 @@ weight per gate row at +-30 / +-100 std (tests/test_weight_distributions_gpu.py 
 
 A variant scheme name ending in "+i8dec" runs the decoder LSTM on int8 slices (mode 2, k_lstm_layer_q8: 16-bit fixed-point
 activations at the fixed scale 32,512, one per-column weight scale over [W_ih | W_hh], a0 x w0 dropped) and every other GEMM
-with the scheme before it, e.g. "f16x3+i8dec".
+with the scheme before it, e.g. "f16x3+i8dec".  A further "+i8lin1" runs linear_1 on int8 slices as well (mode 2, k_gemm_q8: the
+decoder's h quantized to 1 / 32512 steps, one weight scale per output row, a0 x w0 dropped), e.g. "f16x3+i8dec+i8lin1".
+--lin1 replaces linear_1's weights the way --weights replaces the decoder's (one weight per output row at +-3 .. +-100 std for
+the outliers, so that the guard's threshold can be placed between passing and failing estimates; "edge": two
+all-zero rows and two rows scaled by 1e-6), and each line then also prints the guard's estimate for linear_1 (head_err).
 """
 import argparse
 import sys
@@ -62,6 +66,7 @@ class Scheme:
         self.name = name
         self.cache = {}
         self.i8_dec = False
+        self.i8_lin1 = False
 
     def wsplit(self, W, dt, scale=True):
         key = (id(W), dt)
@@ -146,7 +151,9 @@ def variant_forward(S, st, x):
     hid = x
     y = x.flatten(1, 2)
     for i in range(1, 6):
-        y = torch.selu((S.mm(y, st[f"linear_{i}.weight"], slot=3 if i == 1 else 4) + st[f"linear_{i}.bias"].double()).float()).double()
+        W = st[f"linear_{i}.weight"]
+        z = i8_joint(y, W, S) if i == 1 and S.i8_lin1 else S.mm(y, W, slot=3 if i == 1 else 4)
+        y = torch.selu((z + st[f"linear_{i}.bias"].double()).float()).double()
     logits = y.float() @ st["output_layer_type.weight"].float().T + st["output_layer_type.bias"].float()
     return torch.softmax(logits, dim=1), hid
 
@@ -221,32 +228,69 @@ def reweight_decoder(st, dist, seed):
     return st
 
 
+def reweight_lin1(st, dist, seed):
+    """linear_1's weight replaced as --lin1 says (uniform: unchanged)"""
+    if dist == "uniform":
+        return st
+    st = dict(st)
+    rng = np.random.default_rng([seed, 2])
+    W = st["linear_1.weight"].numpy().astype(np.float64)
+    if dist == "t3":
+        X = rng.standard_t(3, size=W.shape)
+        W = X * (W.std() / X.std())
+    elif dist == "edge":
+        W = W.copy()
+        W[[5, 300]] = 0
+        W[[7, 411]] *= 1e-6
+    else:
+        k = float(dist[len("outlier"):])
+        W = W.copy()
+        W[np.arange(W.shape[0]), rng.integers(0, W.shape[1], W.shape[0])] = k * W.std() * rng.choice([-1.0, 1.0], W.shape[0])
+    st["linear_1.weight"] = torch.from_numpy(W.astype(np.float32))
+    return st
+
+
+def head_err(W):
+    """the guard's weight-only estimate for linear_1 (nets_tc.cu pack_q8 with the activation rounding term), largest row"""
+    W = W.to(torch.float64)
+    sw = 32512.0 / torch.where(W.abs().amax(1, keepdim=True) > 0, W.abs().amax(1, keepdim=True), torch.tensor(32512.0, dtype=torch.float64))
+    w1, w0 = q16(W, sw)
+    e = ((256 * w1 + w0) / sw - W).pow(2).sum(1) + 128.0 ** 2 / 3 / 32512.0 ** 2 * (w0 / sw).pow(2).sum(1)
+    e = e + W.pow(2).sum(1) / (12 * 32512.0 ** 2)
+    return e.sqrt().max().item()
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("which", choices=["variant", "polish"])
     ap.add_argument("n", type=int, nargs="?", default=256)
     ap.add_argument("schemes", nargs="?", default="bf16x3,f16x3,f16x2,f16x2a,f16x1,bf16x2")
     ap.add_argument("--weights", choices=["uniform", "t3", "outlier30", "outlier100"], default="uniform")
+    ap.add_argument("--lin1", choices=["uniform", "t3", "outlier3", "outlier4", "outlier6", "outlier9", "outlier30", "outlier100", "edge"],
+                    default="uniform")
     args = ap.parse_args()
     which, n, schemes, dist = args.which, args.n, args.schemes.split(","), args.weights
     if which == "variant":
         for seed in (1, 2):
-            st = reweight_decoder(nets.make_variant_weights(seed), dist, seed)
+            st = reweight_lin1(reweight_decoder(nets.make_variant_weights(seed), dist, seed), args.lin1, seed)
+            he = head_err(st["linear_1.weight"])
             rng = np.random.default_rng(seed)
             x = rng.integers(-40, 41, size=(n, 33, 26)).astype(np.int8)
             x[:, :, 0] = rng.integers(1, 6, size=(n, 33))
             x[rng.random((n, 33, 26)) < 0.5] = 0
             want, whid = nets.variant_predict(st, x, threads=8, return_hidden=True)
             for name in schemes:
-                S = Scheme(name.replace("+i8dec", ""))
-                S.i8_dec = name.endswith("+i8dec")
+                S = Scheme(name.split("+")[0])
+                S.i8_dec = "+i8dec" in name
+                S.i8_lin1 = "+i8lin1" in name
                 p, hid = variant_forward(S, st, torch.from_numpy(x.astype(np.float32)))
                 eh = np.abs(hid.numpy() - whid).max()
                 ep = np.abs(p.numpy() - want).max()
                 srt = np.sort(want, 1)
                 clear = (srt[:, -1] - srt[:, -2]) > 1e-4
                 am = (p.numpy().argmax(1)[clear] != want.argmax(1)[clear]).sum()
-                print(f"variant seed {seed} {dist} {name:8s} max|dh| {eh:.2e}  max|dp| {ep:.2e}  argmax mismatches (clear) {am}", flush=True)
+                print(f"variant seed {seed} {dist} lin1 {args.lin1} {name:8s} max|dh| {eh:.2e}  max|dp| {ep:.2e}  "
+                      f"argmax mismatches (clear) {am}  head_err {he:.2e}", flush=True)
     else:
         for seed in (4, 6):
             st = nets.make_polish_weights(seed)
