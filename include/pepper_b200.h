@@ -591,6 +591,23 @@ int pb_polish_stitch_host(const uint8_t *h_bases, const int64_t *h_position,
                           const int32_t *h_chunk_id, const int64_t *h_region_starts,
                           int64_t n_regions, int64_t n_images, char *h_out,
                           int64_t capacity, int64_t *n_out, void *stream);
+/* The same stitch with the quality of every consensus base: phred [n_images][1000]
+ * is the network's phred (the phred output of pb_polish_call_*); the QV byte of
+ * an output base is '!' + min(phred, 93) of the image column whose base won, so
+ * qual [capacity] lines up with out byte for byte.  out is what
+ * pb_polish_stitch_* writes.                                                    */
+int pb_polish_stitch_qual_device(const uint8_t *d_bases, const uint8_t *d_phred,
+                                 const int64_t *d_position, const int32_t *d_index,
+                                 const int32_t *d_image_region, const int32_t *d_chunk_id,
+                                 const int64_t *d_region_starts, int64_t n_images,
+                                 char *d_out, char *d_qual, int64_t capacity,
+                                 int64_t *n_out, void *stream);
+int pb_polish_stitch_qual_host(const uint8_t *h_bases, const uint8_t *h_phred,
+                               const int64_t *h_position, const int32_t *h_index,
+                               const int32_t *h_image_region, const int32_t *h_chunk_id,
+                               const int64_t *h_region_starts, int64_t n_regions,
+                               int64_t n_images, char *h_out, char *h_qual,
+                               int64_t capacity, int64_t *n_out, void *stream);
 
 /* ------------------------------------------------------------------------
  * Streaming polish session over region GROUPS: make_images + call_consensus + stitch with the consensus written on the
@@ -606,6 +623,10 @@ int pb_polish_stitch_host(const uint8_t *h_bases, const int64_t *h_position,
  * returns PB_ERR_CAPACITY with *n_out = the bytes needed when the sink was too small (restart the session larger).
  * ---------------------------------------------------------------------- */
 int pb_polish_stream_begin(pb_polish_encoder_t *enc, pb_polish_net_t *net, int64_t capacity_bytes, char *d_sink, void *stream);
+/* a session whose sink holds 2-byte records (base, QV byte of pb_polish_stitch_qual_*) in place of bytes: d_sink is
+ * [capacity_records][2]; every count of the session (n_total, n_out, group_bytes) is then in records                  */
+int pb_polish_stream_begin_qual(pb_polish_encoder_t *enc, pb_polish_net_t *net, int64_t capacity_records, char *d_sink,
+                                void *stream);
 int pb_polish_stream_stage_device(pb_polish_encoder_t *enc, const pb_reads_t *d_reads, const pb_region_t *h_regions,
                                   int64_t g0, int64_t g1, int32_t region_id0);
 int pb_polish_stream_run(pb_polish_encoder_t *enc, pb_polish_net_t *net, int flush, int64_t *n_total);
@@ -621,6 +642,12 @@ int pb_test_polish_stitch_sink(const uint8_t *h_bases, const int64_t *h_position
                                const int32_t *h_image_region, const int32_t *h_chunk_id, const int64_t *h_region_starts,
                                int64_t n_regions, int64_t n_images, int64_t chunk, char *h_out, int64_t capacity,
                                int64_t *n_out, int64_t *h_region_bytes, void *stream);
+/* the same with the sink of a pb_polish_stream_begin_qual session: h_records [capacity][2] (base, QV byte)            */
+int pb_test_polish_stitch_sink_qual(const uint8_t *h_bases, const uint8_t *h_phred, const int64_t *h_position,
+                                    const int32_t *h_index, const int32_t *h_image_region, const int32_t *h_chunk_id,
+                                    const int64_t *h_region_starts, int64_t n_regions, int64_t n_images, int64_t chunk,
+                                    char *h_records, int64_t capacity, int64_t *n_out, int64_t *h_region_records,
+                                    void *stream);
 
 /* ------------------------------------------------------------------------
  * Candidate selection (SURVEY 8f row f2).  Replaces the per-candidate logic of

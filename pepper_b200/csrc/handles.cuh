@@ -50,6 +50,7 @@ struct OutSink {
 // one network chunk of polish predictions for the stitch-to-sink kernel (stitch.cu)
 struct SinkArgs {
     const uint8_t *bases = nullptr;                              // [n][1000] network output of the chunk
+    const uint8_t *phred = nullptr;                              // [n][1000] its phred; set: 2-byte (base, QV byte) records
     const int64_t *position = nullptr; const int32_t *index = nullptr;   // [n][1000]
     const int32_t *region = nullptr, *cid = nullptr;             // [n_known] image region / chunk id from the chunk's first image
     const int64_t *start = nullptr;                              // [n] start of each image's region
@@ -57,9 +58,9 @@ struct SinkArgs {
     int64_t n = 0, n_known = 0;
     int32_t prev_region = -1, prev_cid = 0;                      // the image before the chunk (region -1: none)
     int32_t *counts = nullptr; const int64_t *offsets = nullptr; // scratch (set by polish_sink)
-    int64_t *state = nullptr;                                    // [0] running sink offset (bytes needed so far)
-    int64_t *group_bytes = nullptr;
-    char *out = nullptr; int64_t capacity = 0;
+    int64_t *state = nullptr;                                    // [0] running sink offset (records needed so far)
+    int64_t *group_bytes = nullptr;                              // records per slot
+    char *out = nullptr; int64_t capacity = 0;                   // capacity in records
 };
 int polish_sink(SinkArgs A, DevBuf &counts, DevBuf &offsets, cudaStream_t st);
 struct PolishStream;       // streaming polish session state (pipeline.cu)

@@ -585,7 +585,8 @@ struct PolishStream {
     bool active = false;
     cudaStream_t st = nullptr;
     char *d_sink = nullptr;
-    int64_t capacity = 0;
+    int64_t capacity = 0;                       // sink records
+    bool qualities = false;                     // records are (base, QV byte) pairs
     GroupView V[2];
     int32_t region_id0[2] = {0, 0};
     bool staged[2] = {false, false};
@@ -641,8 +642,8 @@ static int psession(pb_polish_encoder_t *e, PolishStream **S, bool need_active) 
     return PB_OK;
 }
 
-extern "C" int pb_polish_stream_begin(pb_polish_encoder_t *e, pb_polish_net_t *net, int64_t capacity_bytes, char *d_sink, void *stream_) {
-    if (!e || !net || (capacity_bytes > 0 && !d_sink)) { set_error("null argument"); return PB_ERR_ARG; }
+static int polish_stream_begin(pb_polish_encoder_t *e, pb_polish_net_t *net, int64_t capacity, char *d_sink, bool qualities, void *stream_) {
+    if (!e || !net || (capacity > 0 && !d_sink)) { set_error("null argument"); return PB_ERR_ARG; }
     PolishStream *S;
     PB_TRY(psession(e, &S, false));
     PB_CUDA(cudaSetDevice(e->device));
@@ -652,7 +653,7 @@ extern "C" int pb_polish_stream_begin(pb_polish_encoder_t *e, pb_polish_net_t *n
     }
     PB_TRY(ensure_events(e->pevt, 3));
     S->st = (cudaStream_t) stream_;
-    S->d_sink = d_sink; S->capacity = std::max<int64_t>(capacity_bytes, 0);
+    S->d_sink = d_sink; S->capacity = std::max<int64_t>(capacity, 0); S->qualities = qualities;
     S->staged[0] = S->staged[1] = false; S->next_stage = 0; S->next_run = 0;
     S->pending = 0; S->h_region.clear(); S->h_cid.clear(); S->prev_region = -1; S->prev_cid = 0;
     S->ev_done = 0; S->enc_ms = S->net_ms = 0.f;
@@ -663,6 +664,16 @@ extern "C" int pb_polish_stream_begin(pb_polish_encoder_t *e, pb_polish_net_t *n
     PB_CUDA(cudaMemsetAsync(S->group_bytes.p, 0, sizeof(int64_t) * S->group_cap, S->st));
     S->active = true;
     return PB_OK;
+}
+
+extern "C" int pb_polish_stream_begin(pb_polish_encoder_t *e, pb_polish_net_t *net, int64_t capacity_bytes, char *d_sink, void *stream_) {
+    return polish_stream_begin(e, net, capacity_bytes, d_sink, false, stream_);
+}
+
+// the same session with a sink of 2-byte (base, QV byte) records: d_sink holds 2 * capacity_records bytes
+extern "C" int pb_polish_stream_begin_qual(pb_polish_encoder_t *e, pb_polish_net_t *net, int64_t capacity_records, char *d_sink,
+                                           void *stream_) {
+    return polish_stream_begin(e, net, capacity_records, d_sink, true, stream_);
 }
 
 // regions [g0, g1) of a workload resident in HBM: only the re-based region rows are copied (copy stream)
@@ -706,6 +717,7 @@ static int polish_stream_network(pb_polish_net_t *net, PolishStream *S, bool flu
         S->net_launches += nl;
         SinkArgs A;
         A.bases = S->bases.as<uint8_t>();
+        A.phred = S->qualities ? S->phred.as<uint8_t>() : nullptr;
         A.position = S->position.as<int64_t>() + done * PB_POLISH_SEQ_LEN; A.index = S->index.as<int32_t>() + done * PB_POLISH_SEQ_LEN;
         A.region = S->region.as<int32_t>() + done; A.cid = S->cid.as<int32_t>() + done;
         A.start = S->start.as<int64_t>() + done; A.slot = S->slot.as<int32_t>() + done;
@@ -800,8 +812,9 @@ extern "C" int pb_polish_stream_sync(pb_polish_encoder_t *e) {
     return PB_OK;
 }
 
-// network + sink over whatever is still pending, wait for everything; *n_out = consensus bytes of the session.  PB_ERR_CAPACITY:
-// the sink was too small, *n_out = the bytes it needed (the bytes past the capacity were not written: restart larger).
+// network + sink over whatever is still pending, wait for everything; *n_out = consensus records of the session (bytes, or
+// (base, QV byte) pairs in a _begin_qual session).  PB_ERR_CAPACITY: the sink was too small, *n_out = the records it needed (the
+// records past the capacity were not written: restart larger).
 extern "C" int pb_polish_stream_end(pb_polish_encoder_t *e, pb_polish_net_t *net, int64_t *n_out) {
     PolishStream *S;
     PB_TRY(psession(e, &S, true));

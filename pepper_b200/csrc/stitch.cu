@@ -24,11 +24,16 @@ __device__ bool str_less(int a, int b) {
     return la < lb;
 }
 
+// FASTQ quality byte of a network phred (0..100): '!' + phred clamped to 93, so that every byte is a printable FASTQ quality
+__device__ __forceinline__ char qv_byte(uint8_t phred) { return (char) ('!' + (phred < 93 ? phred : 93)); }
+
 // The columns of one image that survive (padding, region buffer, the losing side of each chunk overlap, label 0), written in
-// order from out[o0] when WRITE; returns how many survive.  `st` = the start of the image's region.
+// order when WRITE: survivor o's base to out[o * stride] and, given `phred`, its QV byte to qual[o * stride] (o counted from
+// o0; o < capacity).  Returns how many survive.  `st` = the start of the image's region.
 template <bool WRITE>
-__device__ int stitch_columns(const uint8_t *__restrict__ bases, const int64_t *__restrict__ position, const int32_t *__restrict__ index,
-                              int64_t st, bool tail_lost, bool head_lost, char *__restrict__ out, int64_t o0, int64_t capacity) {
+__device__ int stitch_columns(const uint8_t *__restrict__ bases, const uint8_t *__restrict__ phred, const int64_t *__restrict__ position,
+                              const int32_t *__restrict__ index, int64_t st, bool tail_lost, bool head_lost, char *out, char *qual,
+                              int stride, int64_t o0, int64_t capacity) {
     __shared__ int s_warp[8];
     __shared__ int s_carry;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -55,7 +60,10 @@ __device__ int stitch_columns(const uint8_t *__restrict__ bases, const int64_t *
         for (int w = 0; w < warp; w++) base += s_warp[w];
         if (WRITE && keep) {
             const int64_t o = o0 + base + wprefix;
-            if (o < capacity) out[o] = "ACGT"[b - 1];
+            if (o < capacity) {
+                out[o * stride] = "ACGT"[b - 1];
+                if (phred) qual[o * stride] = qv_byte(phred[c]);
+            }
         }
         __syncthreads();
         if (tid == 0) { int s = 0; for (int w = 0; w < 8; w++) s += s_warp[w]; s_carry += s; }
@@ -66,11 +74,11 @@ __device__ int stitch_columns(const uint8_t *__restrict__ bases, const int64_t *
 }
 
 template <bool WRITE>
-__global__ void __launch_bounds__(256) k_stitch(const uint8_t *__restrict__ bases, const int64_t *__restrict__ position,
-                                                const int32_t *__restrict__ index, const int32_t *__restrict__ image_region,
-                                                const int32_t *__restrict__ chunk_id, const int64_t *__restrict__ region_starts,
-                                                int64_t n_images, int32_t *__restrict__ counts, const int64_t *__restrict__ offsets,
-                                                char *__restrict__ out, int64_t capacity) {
+__global__ void __launch_bounds__(256) k_stitch(const uint8_t *__restrict__ bases, const uint8_t *__restrict__ phred,
+                                                const int64_t *__restrict__ position, const int32_t *__restrict__ index,
+                                                const int32_t *__restrict__ image_region, const int32_t *__restrict__ chunk_id,
+                                                const int64_t *__restrict__ region_starts, int64_t n_images, int32_t *__restrict__ counts,
+                                                const int64_t *__restrict__ offsets, char *out, char *qual, int64_t capacity) {
     const int64_t im = blockIdx.x;
     const int reg = image_region[im], cid = chunk_id[im];
     const int64_t st = region_starts[reg];
@@ -79,15 +87,17 @@ __global__ void __launch_bounds__(256) k_stitch(const uint8_t *__restrict__ base
     const bool has_prev = (im > 0) && image_region[im - 1] == reg;
     const bool tail_lost = has_next && str_less(cid, chunk_id[im + 1]);
     const bool head_lost = has_prev && !str_less(chunk_id[im - 1], cid);
-    const int total = stitch_columns<WRITE>(bases + im * SCOLS, position + im * SCOLS, index + im * SCOLS, st, tail_lost, head_lost, out,
-                                            WRITE ? offsets[im] : 0, capacity);
+    const int total = stitch_columns<WRITE>(bases + im * SCOLS, phred ? phred + im * SCOLS : nullptr, position + im * SCOLS,
+                                            index + im * SCOLS, st, tail_lost, head_lost, out, qual, 1, WRITE ? offsets[im] : 0,
+                                            capacity);
     if (!WRITE && threadIdx.x == 0) counts[im] = total;
 }
 
-// Stitch-to-sink: the same rule over one network chunk of a streaming polish session, appended to a byte sink at a running
-// offset that stays on the device.  The neighbours that decide the overlaps may lie outside the chunk: the next image's
-// region / chunk id come from the session's image metadata (known before the network runs, A.n_known images from the chunk's
-// first one), the previous image's from A.prev_region / A.prev_cid.
+// Stitch-to-sink: the same rule over one network chunk of a streaming polish session, appended to a sink at a running record
+// offset that stays on the device.  A record is one consensus byte, or with A.phred the 2 bytes (base, QV byte).  The
+// neighbours that decide the overlaps may lie outside the chunk: the next image's region / chunk id come from the session's
+// image metadata (known before the network runs, A.n_known images from the chunk's first one), the previous image's from
+// A.prev_region / A.prev_cid.
 template <bool WRITE>
 __global__ void __launch_bounds__(256) k_stitch_sink(SinkArgs A) {
     const int64_t im = blockIdx.x;
@@ -96,8 +106,10 @@ __global__ void __launch_bounds__(256) k_stitch_sink(SinkArgs A) {
     const int preg = im > 0 ? A.region[im - 1] : A.prev_region, pcid = im > 0 ? A.cid[im - 1] : A.prev_cid;
     const bool tail_lost = has_next && str_less(cid, A.cid[im + 1]);
     const bool head_lost = preg == reg && !str_less(pcid, cid);
-    const int total = stitch_columns<WRITE>(A.bases + im * SCOLS, A.position + im * SCOLS, A.index + im * SCOLS, A.start[im], tail_lost,
-                                            head_lost, A.out, WRITE ? A.state[0] + A.offsets[im] : 0, A.capacity);
+    const int total = stitch_columns<WRITE>(A.bases + im * SCOLS, A.phred ? A.phred + im * SCOLS : nullptr, A.position + im * SCOLS,
+                                            A.index + im * SCOLS, A.start[im], tail_lost, head_lost, A.out,
+                                            A.phred ? A.out + 1 : nullptr, A.phred ? 2 : 1, WRITE ? A.state[0] + A.offsets[im] : 0,
+                                            A.capacity);
     if (!WRITE && threadIdx.x == 0) {
         A.counts[im] = total;
         if (total) atomicAdd(reinterpret_cast<unsigned long long *>(A.group_bytes + A.slot[im]), (unsigned long long) total);
@@ -125,18 +137,18 @@ int polish_sink(SinkArgs A, DevBuf &counts, DevBuf &offsets, cudaStream_t st) {
 
 using namespace pb;
 
-extern "C" int pb_polish_stitch_device(const uint8_t *d_bases, const int64_t *d_position, const int32_t *d_index,
-                                       const int32_t *d_image_region, const int32_t *d_chunk_id, const int64_t *d_region_starts,
-                                       int64_t n_images, char *d_out, int64_t capacity, int64_t *n_out, void *stream_) {
-    if (!n_out) { set_error("null argument"); return PB_ERR_ARG; }
-    cudaStream_t st = (cudaStream_t) stream_;
+// one-shot stitch of a contig's images: bases to d_out and, given d_phred, QV bytes to d_qual (both [capacity])
+static int stitch_device(const uint8_t *d_bases, const uint8_t *d_phred, const int64_t *d_position, const int32_t *d_index,
+                         const int32_t *d_image_region, const int32_t *d_chunk_id, const int64_t *d_region_starts, int64_t n_images,
+                         char *d_out, char *d_qual, int64_t capacity, int64_t *n_out, cudaStream_t st) {
+    if (!n_out || (d_phred && !d_qual)) { set_error("null argument"); return PB_ERR_ARG; }
     *n_out = 0;
     if (n_images <= 0) return PB_OK;
     DevBuf counts, offsets;
     PB_TRY(counts.reserve(sizeof(int32_t) * n_images));
     PB_TRY(offsets.reserve(sizeof(int64_t) * (n_images + 2)));
-    k_stitch<false><<<(unsigned) n_images, 256, 0, st>>>(d_bases, d_position, d_index, d_image_region, d_chunk_id, d_region_starts, n_images,
-                                                        counts.as<int32_t>(), nullptr, nullptr, 0);
+    k_stitch<false><<<(unsigned) n_images, 256, 0, st>>>(d_bases, nullptr, d_position, d_index, d_image_region, d_chunk_id, d_region_starts,
+                                                        n_images, counts.as<int32_t>(), nullptr, nullptr, nullptr, 0);
     k_scan_excl<<<1, 1024, 0, st>>>(counts.as<int32_t>(), offsets.as<int64_t>(), n_images, offsets.as<int64_t>() + n_images + 1);
     int64_t total = 0;
     PB_CUDA(cudaMemcpyAsync(&total, offsets.as<int64_t>() + n_images, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
@@ -147,8 +159,8 @@ extern "C" int pb_polish_stitch_device(const uint8_t *d_bases, const int64_t *d_
         set_error("consensus capacity %lld < %lld needed", (long long) capacity, (long long) total);
         rc = PB_ERR_CAPACITY;
     } else if (total > 0) {
-        k_stitch<true><<<(unsigned) n_images, 256, 0, st>>>(d_bases, d_position, d_index, d_image_region, d_chunk_id, d_region_starts, n_images,
-                                                           nullptr, offsets.as<int64_t>(), d_out, capacity);
+        k_stitch<true><<<(unsigned) n_images, 256, 0, st>>>(d_bases, d_phred, d_position, d_index, d_image_region, d_chunk_id, d_region_starts,
+                                                           n_images, nullptr, offsets.as<int64_t>(), d_out, d_qual, capacity);
         cudaError_t e = cudaStreamSynchronize(st);
         if (e != cudaSuccess) { set_error("stitch: %s", cudaGetErrorString(e)); rc = PB_ERR_CUDA; }
     }
@@ -156,62 +168,101 @@ extern "C" int pb_polish_stitch_device(const uint8_t *d_bases, const int64_t *d_
     return rc;
 }
 
-extern "C" int pb_polish_stitch_host(const uint8_t *h_bases, const int64_t *h_position, const int32_t *h_index,
-                                     const int32_t *h_image_region, const int32_t *h_chunk_id, const int64_t *h_region_starts,
-                                     int64_t n_regions, int64_t n_images, char *h_out, int64_t capacity, int64_t *n_out, void *stream_) {
-    if (!n_out) { set_error("null argument"); return PB_ERR_ARG; }
+static int stitch_host(const uint8_t *h_bases, const uint8_t *h_phred, const int64_t *h_position, const int32_t *h_index,
+                       const int32_t *h_image_region, const int32_t *h_chunk_id, const int64_t *h_region_starts, int64_t n_regions,
+                       int64_t n_images, char *h_out, char *h_qual, int64_t capacity, int64_t *n_out, cudaStream_t st) {
+    if (!n_out || (h_phred && !h_qual)) { set_error("null argument"); return PB_ERR_ARG; }
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1) { set_error("no CUDA device: libpepper_b200 has no CPU fallback"); return PB_ERR_CUDA; }
-    cudaStream_t st = (cudaStream_t) stream_;
     *n_out = 0;
     if (n_images <= 0) return PB_OK;
-    DevBuf b, p, i, r, c, s, o;
+    const size_t cap = (size_t) std::max<int64_t>(capacity, 1);
+    DevBuf b, p, i, r, c, s, o, ph, q;
     PB_TRY(upload(b, h_bases, (size_t) n_images * SCOLS, st));
     PB_TRY(upload(p, h_position, sizeof(int64_t) * n_images * SCOLS, st));
     PB_TRY(upload(i, h_index, sizeof(int32_t) * n_images * SCOLS, st));
     PB_TRY(upload(r, h_image_region, sizeof(int32_t) * n_images, st));
     PB_TRY(upload(c, h_chunk_id, sizeof(int32_t) * n_images, st));
     PB_TRY(upload(s, h_region_starts, sizeof(int64_t) * n_regions, st));
-    PB_TRY(o.reserve((size_t) std::max<int64_t>(capacity, 1)));
-    int rc = pb_polish_stitch_device(b.as<uint8_t>(), p.as<int64_t>(), i.as<int32_t>(), r.as<int32_t>(), c.as<int32_t>(), s.as<int64_t>(),
-                                     n_images, o.as<char>(), capacity, n_out, stream_);
+    PB_TRY(o.reserve(cap));
+    if (h_phred) {
+        PB_TRY(upload(ph, h_phred, (size_t) n_images * SCOLS, st));
+        PB_TRY(q.reserve(cap));
+    }
+    int rc = stitch_device(b.as<uint8_t>(), h_phred ? ph.as<uint8_t>() : nullptr, p.as<int64_t>(), i.as<int32_t>(), r.as<int32_t>(),
+                           c.as<int32_t>(), s.as<int64_t>(), n_images, o.as<char>(), h_phred ? q.as<char>() : nullptr, capacity, n_out, st);
     if (rc == PB_OK && *n_out > 0) {
         cudaError_t e = cudaMemcpyAsync(h_out, o.p, (size_t) *n_out, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess && h_phred) e = cudaMemcpyAsync(h_qual, q.p, (size_t) *n_out, cudaMemcpyDeviceToHost, st);
         if (e == cudaSuccess) e = cudaStreamSynchronize(st);
         if (e != cudaSuccess) { set_error("stitch copy back: %s", cudaGetErrorString(e)); rc = PB_ERR_CUDA; }
     }
-    DevBuf *bufs[] = {&b, &p, &i, &r, &c, &s, &o};
+    DevBuf *bufs[] = {&b, &p, &i, &r, &c, &s, &o, &ph, &q};
     for (auto *x : bufs) x->release();
     return rc;
 }
 
+extern "C" int pb_polish_stitch_device(const uint8_t *d_bases, const int64_t *d_position, const int32_t *d_index,
+                                       const int32_t *d_image_region, const int32_t *d_chunk_id, const int64_t *d_region_starts,
+                                       int64_t n_images, char *d_out, int64_t capacity, int64_t *n_out, void *stream_) {
+    return stitch_device(d_bases, nullptr, d_position, d_index, d_image_region, d_chunk_id, d_region_starts, n_images, d_out, nullptr,
+                         capacity, n_out, (cudaStream_t) stream_);
+}
+
+extern "C" int pb_polish_stitch_qual_device(const uint8_t *d_bases, const uint8_t *d_phred, const int64_t *d_position,
+                                            const int32_t *d_index, const int32_t *d_image_region, const int32_t *d_chunk_id,
+                                            const int64_t *d_region_starts, int64_t n_images, char *d_out, char *d_qual,
+                                            int64_t capacity, int64_t *n_out, void *stream_) {
+    if (!d_phred) { set_error("null argument"); return PB_ERR_ARG; }
+    return stitch_device(d_bases, d_phred, d_position, d_index, d_image_region, d_chunk_id, d_region_starts, n_images, d_out, d_qual,
+                         capacity, n_out, (cudaStream_t) stream_);
+}
+
+extern "C" int pb_polish_stitch_host(const uint8_t *h_bases, const int64_t *h_position, const int32_t *h_index,
+                                     const int32_t *h_image_region, const int32_t *h_chunk_id, const int64_t *h_region_starts,
+                                     int64_t n_regions, int64_t n_images, char *h_out, int64_t capacity, int64_t *n_out, void *stream_) {
+    return stitch_host(h_bases, nullptr, h_position, h_index, h_image_region, h_chunk_id, h_region_starts, n_regions, n_images, h_out,
+                       nullptr, capacity, n_out, (cudaStream_t) stream_);
+}
+
+extern "C" int pb_polish_stitch_qual_host(const uint8_t *h_bases, const uint8_t *h_phred, const int64_t *h_position,
+                                          const int32_t *h_index, const int32_t *h_image_region, const int32_t *h_chunk_id,
+                                          const int64_t *h_region_starts, int64_t n_regions, int64_t n_images, char *h_out,
+                                          char *h_qual, int64_t capacity, int64_t *n_out, void *stream_) {
+    if (!h_phred) { set_error("null argument"); return PB_ERR_ARG; }
+    return stitch_host(h_bases, h_phred, h_position, h_index, h_image_region, h_chunk_id, h_region_starts, n_regions, n_images, h_out,
+                       h_qual, capacity, n_out, (cudaStream_t) stream_);
+}
+
 // diagnostics: host predictions (images in session order) through the stitch-to-sink kernel `chunk` images at a time, the way a
-// streaming session feeds it one network chunk after the other.  h_region_bytes (optional): bytes per region [n_regions].
-extern "C" int pb_test_polish_stitch_sink(const uint8_t *h_bases, const int64_t *h_position, const int32_t *h_index,
-                                          const int32_t *h_image_region, const int32_t *h_chunk_id, const int64_t *h_region_starts,
-                                          int64_t n_regions, int64_t n_images, int64_t chunk, char *h_out, int64_t capacity,
-                                          int64_t *n_out, int64_t *h_region_bytes, void *stream_) {
+// streaming session feeds it one network chunk after the other.  h_region_bytes (optional): records per region [n_regions].
+// Given h_phred, h_out holds 2-byte (base, QV byte) records [capacity].
+static int stitch_sink_test(const uint8_t *h_bases, const uint8_t *h_phred, const int64_t *h_position, const int32_t *h_index,
+                            const int32_t *h_image_region, const int32_t *h_chunk_id, const int64_t *h_region_starts,
+                            int64_t n_regions, int64_t n_images, int64_t chunk, char *h_out, int64_t capacity,
+                            int64_t *n_out, int64_t *h_region_bytes, cudaStream_t st) {
     if (!n_out || chunk <= 0 || n_regions <= 0) { set_error("bad argument"); return PB_ERR_ARG; }
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1) { set_error("no CUDA device: libpepper_b200 has no CPU fallback"); return PB_ERR_CUDA; }
-    cudaStream_t st = (cudaStream_t) stream_;
     *n_out = 0;
     if (n_images <= 0) return PB_OK;
+    const size_t rec = h_phred ? 2 : 1;
     std::vector<int64_t> start((size_t) n_images);
     for (int64_t i = 0; i < n_images; i++) {
         if (h_image_region[i] < 0 || h_image_region[i] >= n_regions) { set_error("image %lld: region out of range", (long long) i); return PB_ERR_ARG; }
         start[i] = h_region_starts[h_image_region[i]];
     }
-    DevBuf b, p, i, r, c, s, o, state, gb, counts, offsets;
+    DevBuf b, ph, p, i, r, c, s, o, state, gb, counts, offsets;
     int rc = PB_OK;
     do {
         if ((rc = upload(b, h_bases, (size_t) n_images * SCOLS, st)) != PB_OK) break;
+        if (h_phred && (rc = upload(ph, h_phred, (size_t) n_images * SCOLS, st)) != PB_OK) break;
         if ((rc = upload(p, h_position, sizeof(int64_t) * n_images * SCOLS, st)) != PB_OK) break;
         if ((rc = upload(i, h_index, sizeof(int32_t) * n_images * SCOLS, st)) != PB_OK) break;
         if ((rc = upload(r, h_image_region, sizeof(int32_t) * n_images, st)) != PB_OK) break;
         if ((rc = upload(c, h_chunk_id, sizeof(int32_t) * n_images, st)) != PB_OK) break;
         if ((rc = upload(s, start.data(), sizeof(int64_t) * n_images, st)) != PB_OK) break;
-        if ((rc = o.reserve((size_t) std::max<int64_t>(capacity, 1))) != PB_OK) break;
+        if ((rc = o.reserve(rec * (size_t) std::max<int64_t>(capacity, 1))) != PB_OK) break;
         if ((rc = state.reserve(sizeof(int64_t))) != PB_OK) break;
         if ((rc = gb.reserve(sizeof(int64_t) * n_regions)) != PB_OK) break;
         if (cudaMemsetAsync(state.p, 0, sizeof(int64_t), st) != cudaSuccess || cudaMemsetAsync(gb.p, 0, sizeof(int64_t) * n_regions, st) != cudaSuccess) {
@@ -221,6 +272,7 @@ extern "C" int pb_test_polish_stitch_sink(const uint8_t *h_bases, const int64_t 
             SinkArgs A;
             A.n = std::min(chunk, n_images - c0); A.n_known = n_images - c0;
             A.bases = b.as<uint8_t>() + c0 * SCOLS; A.position = p.as<int64_t>() + c0 * SCOLS; A.index = i.as<int32_t>() + c0 * SCOLS;
+            A.phred = h_phred ? ph.as<uint8_t>() + c0 * SCOLS : nullptr;
             A.region = r.as<int32_t>() + c0; A.cid = c.as<int32_t>() + c0; A.start = s.as<int64_t>() + c0; A.slot = r.as<int32_t>() + c0;
             A.prev_region = c0 > 0 ? h_image_region[c0 - 1] : -1; A.prev_cid = c0 > 0 ? h_chunk_id[c0 - 1] : 0;
             A.state = state.as<int64_t>(); A.group_bytes = gb.as<int64_t>(); A.out = o.as<char>(); A.capacity = capacity;
@@ -235,12 +287,30 @@ extern "C" int pb_test_polish_stitch_sink(const uint8_t *h_bases, const int64_t 
         *n_out = total;
         if (total > capacity) { set_error("consensus capacity %lld < %lld needed", (long long) capacity, (long long) total); rc = PB_ERR_CAPACITY; break; }
         if (total > 0) {
-            e = cudaMemcpyAsync(h_out, o.p, (size_t) total, cudaMemcpyDeviceToHost, st);
+            e = cudaMemcpyAsync(h_out, o.p, rec * (size_t) total, cudaMemcpyDeviceToHost, st);
             if (e == cudaSuccess) e = cudaStreamSynchronize(st);
             if (e != cudaSuccess) { set_error("stitch sink copy back: %s", cudaGetErrorString(e)); rc = PB_ERR_CUDA; }
         }
     } while (0);
-    DevBuf *bufs[] = {&b, &p, &i, &r, &c, &s, &o, &state, &gb, &counts, &offsets};
+    DevBuf *bufs[] = {&b, &ph, &p, &i, &r, &c, &s, &o, &state, &gb, &counts, &offsets};
     for (auto *x : bufs) x->release();
     return rc;
+}
+
+extern "C" int pb_test_polish_stitch_sink(const uint8_t *h_bases, const int64_t *h_position, const int32_t *h_index,
+                                          const int32_t *h_image_region, const int32_t *h_chunk_id, const int64_t *h_region_starts,
+                                          int64_t n_regions, int64_t n_images, int64_t chunk, char *h_out, int64_t capacity,
+                                          int64_t *n_out, int64_t *h_region_bytes, void *stream_) {
+    return stitch_sink_test(h_bases, nullptr, h_position, h_index, h_image_region, h_chunk_id, h_region_starts, n_regions, n_images, chunk,
+                            h_out, capacity, n_out, h_region_bytes, (cudaStream_t) stream_);
+}
+
+extern "C" int pb_test_polish_stitch_sink_qual(const uint8_t *h_bases, const uint8_t *h_phred, const int64_t *h_position,
+                                               const int32_t *h_index, const int32_t *h_image_region, const int32_t *h_chunk_id,
+                                               const int64_t *h_region_starts, int64_t n_regions, int64_t n_images, int64_t chunk,
+                                               char *h_records, int64_t capacity, int64_t *n_out, int64_t *h_region_records,
+                                               void *stream_) {
+    if (!h_phred) { set_error("null argument"); return PB_ERR_ARG; }
+    return stitch_sink_test(h_bases, h_phred, h_position, h_index, h_image_region, h_chunk_id, h_region_starts, n_regions, n_images, chunk,
+                            h_records, capacity, n_out, h_region_records, (cudaStream_t) stream_);
 }

@@ -102,9 +102,9 @@ class GroupClaimer:
 
 class GatherBuffer:
     """[world][capacity] records + [world] counts.  A record is `record` (a numpy dtype): the 84-byte prediction record of the
-    variant path by default, one byte of polished consensus for the polish path.  On NCCL the record tensor is allocated from
-    NCCL's own allocator (ncclMemAlloc through torch.cuda.MemPool) when this torch build offers it, so the collective works on
-    registered user buffers; otherwise a plain tensor."""
+    variant path by default, one byte of polished consensus for the polish path (2 bytes, base and quality, with qualities).
+    On NCCL the record tensor is allocated from NCCL's own allocator (ncclMemAlloc through torch.cuda.MemPool) when this torch
+    build offers it, so the collective works on registered user buffers; otherwise a plain tensor."""
 
     def __init__(self, capacity: int, world: int, rank: int, device=None, max_groups: int = 0, record=PRED_RECORD):
         import torch
@@ -360,7 +360,8 @@ class _RankDriver:
         return GroupClaimer(n_job, self.rank, self.world, self.schedule, work, key="%s_%d" % (self._claim_prefix, self._calls))
 
     def _gather_buffer(self, capacity: int, n_job: int, record=PRED_RECORD) -> GatherBuffer:
-        if self.buffer is None or self.buffer.max_groups < n_job or self.buffer.capacity != capacity:
+        if (self.buffer is None or self.buffer.max_groups < n_job or self.buffer.capacity != capacity
+                or self.buffer.record != np.dtype(record)):
             if self.buffer is not None:
                 self.buffer.release()
             self.buffer = GatherBuffer(capacity, self.world, self.rank, self.device, max_groups=n_job, record=record)
@@ -487,23 +488,30 @@ class DistributedPolisher(_RankDriver):
 
     `capacity_bytes`: this rank's slice of the gather buffer; a rank stops claiming groups when the columns it has encoded (an
     upper bound of its consensus bytes) leave too little room, and run() fails if the ranks together could not run every
-    group.  `distributed=False` runs the same path on this process alone (world size 1)."""
+    group.  `distributed=False` runs the same path on this process alone (world size 1).
+
+    `qualities=True`: the session writes 2-byte polish.QUAL_RECORD records (base, FASTQ quality byte) in place of bytes, still
+    gathered by one all-gather; `capacity_bytes` then counts records (consensus bases) and assemble() returns
+    {contig: (sequence, quality string)}."""
 
     _claim_prefix = "pb_polish_claim"
 
     def __init__(self, state: dict, device: int, capacity_bytes: int, schedule: str = "dynamic", group_regions: int = 32,
-                 distributed: bool = True, caller=None):
+                 distributed: bool = True, caller=None, qualities: bool = False):
         from .pipeline import PolishCaller
         super().__init__(PolishCaller, state, device, schedule, group_regions, distributed, caller)
         self.capacity = int(capacity_bytes)
+        self.qualities = bool(qualities)
 
     def run(self, source) -> int:
-        """Returns this rank's consensus bytes; the gathered bytes of every rank are in self.buffer (device)."""
+        """Returns this rank's consensus bytes (records with qualities); the gathered records of every rank are in self.buffer
+        (device)."""
+        from .polish import QUAL_RECORD
         groups = source.groups(self.group_regions)
         n_job = len(groups)
-        self._gather_buffer(self.capacity, n_job, np.uint8)
+        self._gather_buffer(self.capacity, n_job, QUAL_RECORD if self.qualities else np.uint8)
         claimer = self._claimer(n_job, source.group_work(groups))
-        s = self.caller.stream(self.capacity, self.buffer.my_ptr())
+        s = self.caller.stream(self.capacity, self.buffer.my_ptr(), qualities=self.qualities)
         segments = self._run_job(s, claimer, groups, self.capacity, source)
         n = s.end()
         segments = [(g, int(k)) for (g, _), k in zip(segments, s.group_bytes())]
@@ -512,21 +520,29 @@ class DistributedPolisher(_RankDriver):
 
     def assemble(self, source) -> dict:
         """{contig: polished sequence} of every contig of the source's plan (empty string: nothing survived), on every rank:
-        the gathered bytes in group order, cut at the contig boundaries of the plan."""
+        the gathered bytes in group order, cut at the contig boundaries of the plan.  With qualities: {contig: (sequence,
+        quality string)}."""
         groups = source.groups(self.group_regions)
         return assemble_contigs(self.buffer.to_host(), self.buffer.segments(), [source.names[source.contig_of[g0]] for g0, _ in groups],
                                 source.names)
 
 
 def assemble_contigs(data: np.ndarray, segments: list[tuple[int, int]], group_contig: list[str], contigs: list[str]) -> dict:
-    """Consensus bytes `data` of the groups of `segments` ((group id, bytes), sorted by group id, laid out in that order) ->
-    {contig: sequence} for every contig of `contigs` (group g belongs to contig group_contig[g])."""
-    parts = {c: [] for c in contigs}
+    """Consensus records `data` of the groups of `segments` ((group id, records), sorted by group id, laid out in that order) ->
+    {contig: sequence} for every contig of `contigs` (group g belongs to contig group_contig[g]).  Records are bytes, or
+    (base, qual) records (polish.QUAL_RECORD), which give {contig: (sequence, quality string)}."""
+    spans = {c: [] for c in contigs}
     off = 0
     for g, k in segments:
-        parts[group_contig[g]].append(bytes(data[off:off + k]))
+        spans[group_contig[g]].append((off, off + k))
         off += k
-    return {c: b"".join(p).decode() for c, p in parts.items()}
+
+    def cut(plane: bytes) -> dict:
+        return {c: b"".join(plane[a:b] for a, b in sp).decode() for c, sp in spans.items()}
+    if data.dtype.names is None:
+        return cut(data.tobytes())
+    seqs, quals = cut(data["base"].tobytes()), cut(data["qual"].tobytes())
+    return {c: (seqs[c], quals[c]) for c in contigs}
 
 
 # ---------------------------------------------------------------------------------------------------------------------------

@@ -564,10 +564,11 @@ class PolishFromFiles(_FromFiles):
         return PolishCalls(h["bases"], h["phred"], h["position"], h["index"], h["image_region"], h["chunk_id"]), fetched_table(fetched, regions)
 
     def polish_contig(self, contig: str, start: int = 0, end: int | None = None, batch: int = 2000, realign: bool = True,
-                      return_calls: bool = False):
+                      return_calls: bool = False, qualities: bool = False):
         """The whole polish path of one contig span: tiling (ImageGenerationUI.py:262-272: the span is [start, length - 1]),
-        make_images + call_consensus in batches of `batch` regions, then the stitch (Stitch.py:36-128) -> polished sequence."""
-        from .polish import stitch
+        make_images + call_consensus in batches of `batch` regions, then the stitch (Stitch.py:36-128) -> polished sequence;
+        `qualities`: (sequence, FASTQ quality string) (polish.stitch_with_qualities).  `return_calls`: (that, calls, regions)."""
+        from .polish import stitch, stitch_with_qualities
         if end is None:
             end = self.fasta.get_chromosome_sequence_length(contig) - 1
         regs = polish_intervals(start, end)
@@ -578,21 +579,28 @@ class PolishFromFiles(_FromFiles):
         cat = lambda f: np.concatenate([getattr(c, f) for c, _ in parts])       # noqa: E731
         image_region = np.concatenate([c.image_region + off for c, off in parts]).astype(np.int32)
         allc = PolishCalls(cat("bases"), cat("phred"), cat("position"), cat("index"), image_region, cat("chunk_id"))
-        seq = stitch(allc.bases, allc.position, allc.index, allc.image_region, allc.chunk_id, np.array([r[0] for r in regs], dtype=np.int64))
+        starts = np.array([r[0] for r in regs], dtype=np.int64)
+        if qualities:
+            seq = stitch_with_qualities(allc.bases, allc.phred, allc.position, allc.index, allc.image_region, allc.chunk_id, starts)
+        else:
+            seq = stitch(allc.bases, allc.position, allc.index, allc.image_region, allc.chunk_id, starts)
         return (seq, allc, regs) if return_calls else seq
 
     def polish_assembly(self, out_path: str | None = None, contigs: list[str] | None = None, group_regions: int = 32,
-                        capacity_bytes: int | None = None, realign: bool = True) -> dict:
+                        capacity_bytes: int | None = None, realign: bool = True, fastq: bool = False) -> dict:
         """`pepper polish` of a whole assembly on this GPU: every contig common to the BAM and the FASTA (or `contigs`),
         make_images + call_consensus + the stitch on the device through one streaming session (dist.DistributedPolisher at world
-        size 1).  Returns {contig: polished sequence} and, given `out_path`, writes the FASTA perform_stitch writes."""
+        size 1).  Returns {contig: polished sequence} and, given `out_path`, writes the FASTA perform_stitch writes.
+        `fastq`: the quality of every base is carried through the stitch; returns {contig: (sequence, quality string)} and
+        writes FASTQ (write_polished_fastq) to `out_path`."""
         from .dist import DistributedPolisher
         src = PolishFileSource(self.bam.path, self.fasta_path, contigs, self.device, self.threads, self.gpu_inflate, realign,
                                host_share=self.host_share)
         try:
             cap = capacity_bytes or 2 * sum(e - s + 1 for s, e in src.intervals) + (1 << 20)
             while True:
-                dp = DistributedPolisher(None, self.device, cap, "static", group_regions, distributed=False, caller=self.caller)
+                dp = DistributedPolisher(None, self.device, cap, "static", group_regions, distributed=False, caller=self.caller,
+                                         qualities=fastq)
                 try:
                     dp.run(src)
                     seqs = dp.assemble(src)
@@ -606,7 +614,7 @@ class PolishFromFiles(_FromFiles):
         finally:
             src.close()
         if out_path is not None:
-            write_polished_fasta(out_path, seqs)
+            (write_polished_fastq if fastq else write_polished_fasta)(out_path, seqs)
         return seqs
 
 
@@ -625,6 +633,21 @@ def write_polished_fasta(path: str, seqs: dict) -> None:
 
 def polished_fasta_text(seqs: dict) -> str:
     return "".join(">%s\n%s\n" % (c, seqs[c]) for c in sorted(seqs, key=natural_key) if seqs[c])
+
+
+def write_polished_fastq(path: str, records: dict) -> None:
+    """The polished assembly with the quality of every base: '@contig\n<sequence>\n+\n<qualities>\n' per contig, no line
+    wrapping, contigs in natural order, contigs with an empty consensus left out (the contigs and sequences of
+    write_polished_fasta).  `records`: {contig: (sequence, quality string)}."""
+    with open(path, "w") as f:
+        f.write(polished_fastq_text(records))
+
+
+def polished_fastq_text(records: dict) -> str:
+    for c, (seq, qual) in records.items():
+        if len(seq) != len(qual):
+            raise ValueError("%s: %d bases but %d qualities" % (c, len(seq), len(qual)))
+    return "".join("@%s\n%s\n+\n%s\n" % ((c,) + tuple(records[c])) for c in sorted(records, key=natural_key) if records[c][0])
 
 
 def polish_job(fasta_contigs: list[tuple[str, int]], bam_contigs: list[str], contigs: list[str] | None = None,

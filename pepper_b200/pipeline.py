@@ -79,6 +79,7 @@ def _bind_calls(L):
                                         vp, vp, vp, vp, C.POINTER(C.c_int64), vp]
     L.pb_polish_call_timings.argtypes = [vp, vp]
     L.pb_polish_stream_begin.argtypes = [vp, vp, C.c_int64, vp, vp]
+    L.pb_polish_stream_begin_qual.argtypes = [vp, vp, C.c_int64, vp, vp]
     L.pb_polish_stream_stage_device.argtypes = [vp, C.POINTER(PbReads), C.POINTER(PbRegion), C.c_int64, C.c_int64, C.c_int32]
     L.pb_polish_stream_run.argtypes = [vp, vp, C.c_int, C.POINTER(C.c_int64)]
     L.pb_polish_stream_sync.argtypes = [vp]
@@ -338,9 +339,9 @@ class PolishCaller:
         return d
 
 
-    def stream(self, capacity_bytes: int, d_sink: int, stream: int = 0) -> "PolishStream":
+    def stream(self, capacity_bytes: int, d_sink: int, stream: int = 0, qualities: bool = False) -> "PolishStream":
         """Streaming session over region groups with the stitch on the device (pb_polish_stream_*): see PolishStream."""
-        return PolishStream(self, capacity_bytes, d_sink, stream)
+        return PolishStream(self, capacity_bytes, d_sink, stream, qualities)
 
 
 class PolishStream:
@@ -356,14 +357,17 @@ class PolishStream:
             s.stage_device(...)
         n = s.end()                      # bytes written; PepperB200Error(PB_ERR_CAPACITY) when the sink was too small
         per_group = s.group_bytes()      # bytes of each group, in run order
-    """
 
-    def __init__(self, caller: PolishCaller, capacity_bytes: int, d_sink: int, stream: int = 0):
+    `qualities=True` (pb_polish_stream_begin_qual): the sink holds 2-byte polish.QUAL_RECORD records (base, FASTQ quality
+    byte) in place of bytes, `d_sink` is 2 * `capacity_bytes` bytes, and every count of the session is in records."""
+
+    def __init__(self, caller: PolishCaller, capacity_bytes: int, d_sink: int, stream: int = 0, qualities: bool = False):
         self.c, self.L = caller, caller.L
         self.capacity = int(capacity_bytes)
         self.groups = 0
-        _lib.check(self.L.pb_polish_stream_begin(caller.enc.h, caller.net.h, self.capacity, C.c_void_p(d_sink or None),
-                                                 C.c_void_p(stream)), "pb_polish_stream_begin")
+        begin = self.L.pb_polish_stream_begin_qual if qualities else self.L.pb_polish_stream_begin
+        _lib.check(begin(caller.enc.h, caller.net.h, self.capacity, C.c_void_p(d_sink or None), C.c_void_p(stream)),
+                   "pb_polish_stream_begin_qual" if qualities else "pb_polish_stream_begin")
 
     def stage_device(self, dreads, g0: int, g1: int, region_id0: int = 0):
         """`dreads`: DeviceReads / FetchedReads whose region table the group indices [g0, g1) refer to."""

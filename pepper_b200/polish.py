@@ -16,6 +16,8 @@ from .abi import HostReads, PbReads, PbRegion, regions_array, POLISH_FEATURES, P
 from .synth import ReadBatch, RegionTable
 
 SEQ_OVERLAP = 50      # pepper Options.py ImageSizeOptions.SEQ_OVERLAP
+# one consensus base of a qualities sink (pb_polish_stream_begin_qual): the base letter and its FASTQ quality byte
+QUAL_RECORD = np.dtype([("base", "u1"), ("qual", "u1")])
 
 
 @dataclass
@@ -198,14 +200,42 @@ def stitch(bases, position, index, image_region, chunk_id, region_starts, stream
     return bytes(out[:int(n.value)]).decode()
 
 
-def stitch_sink_test(bases, position, index, image_region, chunk_id, region_starts, chunk: int, stream: int = 0):
-    """Diagnostics (pb_test_polish_stitch_sink): the predictions of images in session order through the streaming session's
-    stitch-to-sink kernel, `chunk` images per call.  Returns (consensus str, bytes per region int64 [n_regions])."""
+def stitch_with_qualities(bases, phred, position, index, image_region, chunk_id, region_starts, stream: int = 0) -> tuple[str, str]:
+    """`stitch` with the quality of every consensus base, on the GPU: (sequence, FASTQ quality string).  The QV of a base is
+    the network phred of the image column whose base won the stitch, written as '!' + min(phred, 93); the sequence is what
+    `stitch` returns."""
     _lib.require_gpu()
     L = _lib.lib()
     vp = C.c_void_p
-    L.pb_test_polish_stitch_sink.argtypes = [vp, vp, vp, vp, vp, vp, C.c_int64, C.c_int64, C.c_int64, vp, C.c_int64,
-                                             C.POINTER(C.c_int64), vp, vp]
+    L.pb_polish_stitch_qual_host.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.c_int64, C.c_int64, vp, vp, C.c_int64, C.POINTER(C.c_int64), vp]
+    b = np.ascontiguousarray(bases, dtype=np.uint8)
+    q = np.ascontiguousarray(phred, dtype=np.uint8)
+    p = np.ascontiguousarray(position, dtype=np.int64)
+    i = np.ascontiguousarray(index, dtype=np.int32)
+    r = np.ascontiguousarray(image_region, dtype=np.int32)
+    c = np.ascontiguousarray(chunk_id, dtype=np.int32)
+    s = np.ascontiguousarray(region_starts, dtype=np.int64)
+    if q.shape != b.shape:
+        raise ValueError("phred shape %s != bases shape %s" % (q.shape, b.shape))
+    n_img = b.shape[0]
+    cap = max(1, n_img * POLISH_SEQ_LEN)
+    out = np.empty(cap, dtype=np.uint8)
+    qual = np.empty(cap, dtype=np.uint8)
+    n = C.c_int64(0)
+    _lib.check(L.pb_polish_stitch_qual_host(b.ctypes.data, q.ctypes.data, p.ctypes.data, i.ctypes.data, r.ctypes.data, c.ctypes.data,
+                                            s.ctypes.data, s.shape[0], n_img, out.ctypes.data, qual.ctypes.data, cap, C.byref(n),
+                                            C.c_void_p(stream)), "pb_polish_stitch_qual_host")
+    k = int(n.value)
+    return bytes(out[:k]).decode(), bytes(qual[:k]).decode()
+
+
+def stitch_sink_test(bases, position, index, image_region, chunk_id, region_starts, chunk: int, stream: int = 0, phred=None):
+    """Diagnostics (pb_test_polish_stitch_sink): the predictions of images in session order through the streaming session's
+    stitch-to-sink kernel, `chunk` images per call.  Returns (consensus str, bytes per region int64 [n_regions]); given `phred`
+    (pb_test_polish_stitch_sink_qual: the sink of a qualities session), ((consensus str, quality str), records per region)."""
+    _lib.require_gpu()
+    L = _lib.lib()
+    vp = C.c_void_p
     b = np.ascontiguousarray(bases, dtype=np.uint8)
     p = np.ascontiguousarray(position, dtype=np.int64)
     i = np.ascontiguousarray(index, dtype=np.int32)
@@ -213,10 +243,28 @@ def stitch_sink_test(bases, position, index, image_region, chunk_id, region_star
     c = np.ascontiguousarray(chunk_id, dtype=np.int32)
     s = np.ascontiguousarray(region_starts, dtype=np.int64)
     cap = max(1, b.shape[0] * POLISH_SEQ_LEN)
-    out = np.empty(cap, dtype=np.uint8)
     per_region = np.zeros(s.shape[0], np.int64)
     n = C.c_int64(0)
-    _lib.check(L.pb_test_polish_stitch_sink(b.ctypes.data, p.ctypes.data, i.ctypes.data, r.ctypes.data, c.ctypes.data, s.ctypes.data,
-                                            s.shape[0], b.shape[0], int(chunk), out.ctypes.data, cap, C.byref(n), per_region.ctypes.data,
-                                            C.c_void_p(stream)), "pb_test_polish_stitch_sink")
-    return bytes(out[:int(n.value)]).decode(), per_region
+    if phred is None:
+        L.pb_test_polish_stitch_sink.argtypes = [vp, vp, vp, vp, vp, vp, C.c_int64, C.c_int64, C.c_int64, vp, C.c_int64,
+                                                 C.POINTER(C.c_int64), vp, vp]
+        out = np.empty(cap, dtype=np.uint8)
+        _lib.check(L.pb_test_polish_stitch_sink(b.ctypes.data, p.ctypes.data, i.ctypes.data, r.ctypes.data, c.ctypes.data, s.ctypes.data,
+                                                s.shape[0], b.shape[0], int(chunk), out.ctypes.data, cap, C.byref(n), per_region.ctypes.data,
+                                                C.c_void_p(stream)), "pb_test_polish_stitch_sink")
+        return bytes(out[:int(n.value)]).decode(), per_region
+    L.pb_test_polish_stitch_sink_qual.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.c_int64, C.c_int64, C.c_int64, vp, C.c_int64,
+                                                  C.POINTER(C.c_int64), vp, vp]
+    q = np.ascontiguousarray(phred, dtype=np.uint8)
+    if q.shape != b.shape:
+        raise ValueError("phred shape %s != bases shape %s" % (q.shape, b.shape))
+    rec = np.empty(cap, dtype=QUAL_RECORD)
+    _lib.check(L.pb_test_polish_stitch_sink_qual(b.ctypes.data, q.ctypes.data, p.ctypes.data, i.ctypes.data, r.ctypes.data, c.ctypes.data,
+                                                 s.ctypes.data, s.shape[0], b.shape[0], int(chunk), rec.ctypes.data, cap, C.byref(n),
+                                                 per_region.ctypes.data, C.c_void_p(stream)), "pb_test_polish_stitch_sink_qual")
+    return split_records(rec[:int(n.value)]), per_region
+
+
+def split_records(rec: np.ndarray) -> tuple[str, str]:
+    """(base, qual) records of a qualities sink -> (sequence, quality string)."""
+    return rec["base"].tobytes().decode(), rec["qual"].tobytes().decode()

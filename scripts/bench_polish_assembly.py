@@ -7,7 +7,12 @@ Prints one JSON line: polished bases/s (consensus bytes of the whole assembly pe
 bases/s, per-rank encoder / network / wait / gather ms and groups, the card name and its power limit.  Rank 0 checks the
 assembly against the single-GPU `polish_contig` of sampled contigs (`verified`).
 
-    python scripts/bench_polish_assembly.py [--contigs 20] [--mb 5] [--coverage 40] [--group-regions 32] [--check 3]"""
+`--fastq`: after the timed run above, the same assembly is polished `--reps` more times with and `--reps` times without
+per-base qualities, the two modes alternating on one driver, and the line gains `fastq`: the wall time of every run, the
+polished bases/s of each mode (total bases over total wall), and whether the FASTQ sequences equal the FASTA sequences.
+
+    python scripts/bench_polish_assembly.py [--contigs 20] [--mb 5] [--coverage 40] [--group-regions 32] [--check 3]
+                                            [--fastq [--reps 3]]"""
 import argparse
 import json
 import os
@@ -56,6 +61,8 @@ def main():
     ap.add_argument("--schedule", default="dynamic")
     ap.add_argument("--check", type=int, default=3, help="contigs compared with polish_contig on rank 0")
     ap.add_argument("--seed", type=int, default=1)
+    ap.add_argument("--fastq", action="store_true", help="also time the assembly with per-base qualities, alternating with FASTA")
+    ap.add_argument("--reps", type=int, default=3, help="--fastq: runs of each mode")
     args = ap.parse_args()
 
     import torch
@@ -81,17 +88,37 @@ def main():
         # warm-up on one contig: library buffers, first kernel launches, NCCL communicator
         wsrc = PolishFileSource(bam, fa, contigs=names[:1], device=local)
         dp = DistributedPolisher(state, local, cap, args.schedule, args.group_regions)
-        dp.run(wsrc)
+        for q in ([False, True] if args.fastq else [False]):
+            dp.qualities = q
+            dp.run(wsrc)
+        dp.qualities = False
         wsrc.close()
         src = PolishFileSource(bam, fa, device=local)
-        if world > 1:
-            dist.barrier()
-        torch.cuda.synchronize()
-        t1 = time.perf_counter()
-        n = dp.run(src)
-        seqs = dp.assemble(src)
-        wall = time.perf_counter() - t1
+
+        def timed(qualities: bool):
+            dp.qualities = qualities
+            if world > 1:
+                dist.barrier()
+            torch.cuda.synchronize()
+            t = time.perf_counter()
+            n = dp.run(src)
+            out = dp.assemble(src)
+            return n, out, time.perf_counter() - t
+        n, seqs, wall = timed(False)
         mine = dict(dp.phase_ms, consensus_bytes=n, images=dp.stats.get("images", 0))
+        fastq = None
+        if args.fastq:
+            walls = {"fasta": [], "fastq": []}
+            same = True
+            for rep in range(args.reps):
+                for q in ((True, False) if rep % 2 == 0 else (False, True)):
+                    _, out, w = timed(q)
+                    walls["fastq" if q else "fasta"].append(w)
+                    same = same and ({c: s for c, (s, _) in out.items()} if q else out) == seqs
+            bases = sum(len(s) for s in seqs.values())
+            fastq = dict(reps=args.reps, wall_s={k: [round(w, 3) for w in v] for k, v in walls.items()},
+                         polished_bases_per_s={k: round(bases * len(v) / sum(v), 1) for k, v in walls.items()},
+                         fastq_sequences_equal_fasta=bool(same))
         per_rank = [None] * world
         if world > 1:
             dist.all_gather_object(per_rank, mine)
@@ -115,7 +142,7 @@ def main():
                 wall_s=round(wall, 3), polished_bases_per_s=round(polished / wall, 1), draft_bases_per_s=round(draft / wall, 1),
                 per_rank=[{k: (round(v, 2) if isinstance(v, float) else v) for k, v in r.items()} for r in per_rank],
                 card=torch.cuda.get_device_name(local), power_limit_w=power_limit_w(local), synth_s=round(gen_s, 1),
-                verified=verified)), flush=True)
+                verified=verified, **({"fastq": fastq} if args.fastq else {}))), flush=True)
     finally:
         shutil.rmtree(tmp, ignore_errors=True)
         if world > 1:
