@@ -875,42 +875,48 @@ class DistributedGenomeCaller(_RankDriver):
     def call_genome(self, bam: str, fasta: str, out_dir: str, sample_name: str, region: str | None = None, exclude=(),
                     params: dict | None = None, options: dict | None = None, vcf_options: dict | None = None,
                     interval_size: int = 100_000, gpu_inflate: bool = True) -> tuple:
-        import time
         from .frontend import VariantGenomeSource
         from .synth import ont_params
-        from .vcf import write_vcfs_from_parts
         params = params or ont_params()
         src = VariantGenomeSource(bam, fasta, int(params["min_snp_baseq"]), region, exclude, interval_size, self.device_id,
                                   gpu_inflate=gpu_inflate)
         try:
-            groups = src.groups(self.group_regions)
-            part = self.run_groups(src, self._claimer(len(groups), src.group_work(groups)), params, options, vcf_options)
-            t0 = time.perf_counter()
-            held = self._all_gather_object(part.held)
-            held = np.concatenate(held) if held else np.zeros(0, PRED_RECORD)
-            part.phase_ms["edge_exchange"] = (time.perf_counter() - t0) * 1e3
-            self.edge_pass(part, src, held, options, vcf_options)
-            table = sum(self._all_gather_object(group_table_rows(part, len(groups))))
-            check_groups_ran(int(table[:, GT_RAN].sum()), len(groups), "the session capacity (%d bytes per rank)" % self.capacity,
-                             "capacity_bytes")
-            totals = self.compress(part, src, table)
-            t0 = time.perf_counter()
-            got = self._gather_bytes(part)
-            part.phase_ms["gather"] = (time.perf_counter() - t0) * 1e3
-            t0 = time.perf_counter()
-            if got is not None:
-                parts = {}
-                for data in got:
-                    parts.update(parse_rank_bytes(data))
-                write_vcfs_from_parts(out_dir, sample_name, src.fasta_contigs(), src.names,
-                                      [int(src.contig_of[g0]) for g0, _ in groups], parts)
-            part.phase_ms["write"] = (time.perf_counter() - t0) * 1e3
-            part.phase_ms["groups"] = len(part.groups)
-            self.phase_ms = {k: round(v, 2) for k, v in part.phase_ms.items()}
-            self.payload_bytes, self.member_bytes = part.payload_bytes, int(part.comp.shape[0])
-            return totals
+            return self.call_source(src, out_dir, sample_name, params, options, vcf_options)
         finally:
             src.close()
+
+    def call_source(self, src, out_dir: str, sample_name: str, params: dict, options: dict | None = None,
+                    vcf_options: dict | None = None) -> tuple:
+        """call_genome over a read source the caller opened (frontend.VariantGenomeSource, with its own get_reads filters and
+        BAM threads); every rank passes a source of the same job.  The source stays open."""
+        import time
+        from .vcf import write_vcfs_from_parts
+        groups = src.groups(self.group_regions)
+        part = self.run_groups(src, self._claimer(len(groups), src.group_work(groups)), params, options, vcf_options)
+        t0 = time.perf_counter()
+        held = self._all_gather_object(part.held)
+        held = np.concatenate(held) if held else np.zeros(0, PRED_RECORD)
+        part.phase_ms["edge_exchange"] = (time.perf_counter() - t0) * 1e3
+        self.edge_pass(part, src, held, options, vcf_options)
+        table = sum(self._all_gather_object(group_table_rows(part, len(groups))))
+        check_groups_ran(int(table[:, GT_RAN].sum()), len(groups), "the session capacity (%d bytes per rank)" % self.capacity,
+                         "capacity_bytes")
+        totals = self.compress(part, src, table)
+        t0 = time.perf_counter()
+        got = self._gather_bytes(part)
+        part.phase_ms["gather"] = (time.perf_counter() - t0) * 1e3
+        t0 = time.perf_counter()
+        if got is not None:
+            parts = {}
+            for data in got:
+                parts.update(parse_rank_bytes(data))
+            write_vcfs_from_parts(out_dir, sample_name, src.fasta_contigs(), src.names,
+                                  [int(src.contig_of[g0]) for g0, _ in groups], parts)
+        part.phase_ms["write"] = (time.perf_counter() - t0) * 1e3
+        part.phase_ms["groups"] = len(part.groups)
+        self.phase_ms = {k: round(v, 2) for k, v in part.phase_ms.items()}
+        self.payload_bytes, self.member_bytes = part.payload_bytes, int(part.comp.shape[0])
+        return totals
 
 
 def _device_column(ptr: int, shape: tuple, typestr: str, device):

@@ -654,18 +654,25 @@ def polish_job(fasta_contigs: list[tuple[str, int]], bam_contigs: list[str], con
                max_end: int | None = None):
     """The job of a whole-assembly polish: every contig common to the FASTA (name, length) and the BAM, in natural order
     (ImageGenerationUI.get_chromosome_list, pepper ImageGenerationUI.py:88-117), or `contigs`; each contig tiled with
-    polish_intervals(0, length - 1) (a contig too short to tile has no region).  Returns (contigs, regions laid out contig after
-    contig, first region of each contig + the total).  `max_end`: the BAM index's reach; a longer contig raises ValueError."""
+    polish_intervals(0, length - 1) (a contig too short to tile has no region).  An entry of `contigs` may also be
+    (contig, (start, end)) or (contig, None), as parse_region gives them: that contig is tiled over [max(0, start),
+    min(end, length - 1)] (pepper ImageGenerationUI.py:257-272).  Returns (contigs, regions laid out contig after contig, first
+    region of each contig + the total).  `max_end`: the BAM index's reach; a longer contig raises ValueError."""
     lengths = dict(fasta_contigs)
     if contigs is None:
         contigs = sorted(set(lengths) & set(bam_contigs), key=natural_key)
-    check_reach([(c, lengths[c]) for c in contigs if c in lengths], max_end)
-    regions, first = [], []
+    spans = []
     for c in contigs:
+        c, span = (c, None) if isinstance(c, str) else c
+        s, e = span if span is not None else (0, lengths[c] - 1)
+        spans.append((c, max(0, s), min(e, lengths[c] - 1)))
+    check_reach([(c, e + 1) for c, _, e in spans], max_end)
+    regions, first = [], []
+    for _, s, e in spans:
         first.append(len(regions))
-        regions.extend(polish_intervals(0, lengths[c] - 1))
+        regions.extend(polish_intervals(s, e))
     first.append(len(regions))
-    return list(contigs), regions, first
+    return [c for c, _, _ in spans], regions, first
 
 
 def parse_region(region: str) -> list[tuple[str, tuple[int, int] | None]]:
@@ -730,7 +737,7 @@ def variant_job(fasta_contigs: list[tuple[str, int]], bam_contigs: list[str], re
 class PolishFileSource(_GroupSource):
     """The read source of dist.DistributedPolisher: a whole assembly, every contig common to both files in natural order
     (ImageGenerationUI.get_chromosome_list, pepper ImageGenerationUI.py:88-117) or the given `contigs`, each tiled with
-    polish_intervals(0, length - 1).  `take` runs get_reads with the filters of PolishFromFiles.call and the realignment on a
+    polish_intervals(0, length - 1), or over its span where `contigs` gives one (polish_job).  `take` runs get_reads with the filters of PolishFromFiles.call and the realignment on a
     side stream, so that a group's inflate, trim and realignment run beside the previous group's network."""
 
     def __init__(self, bam_path: str, fasta_path: str, contigs: list[str] | None = None, device: int = 0, threads: int = 0,
