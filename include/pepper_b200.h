@@ -650,6 +650,55 @@ int pb_test_polish_stitch_sink_qual(const uint8_t *h_bases, const uint8_t *h_phr
                                     void *stream);
 
 /* ------------------------------------------------------------------------
+ * Polish edits: what the stitch changed in the draft.  An edits session (pb_polish_stream_edits after _begin or _begin_qual)
+ * writes, beside the consensus, one event per winning image column that is not an identity (the stitch's winner of (position,
+ * index) taken before label-0 columns are dropped): a deletion (label 0 at index 0), a substitution (a label other than the
+ * upper-cased draft base at index 0) or an insertion (index >= 1, label other than 0); and per image one coverage record: the
+ * first and last index-0 position it won.  Events of an image follow its columns' order, its coverage record comes last; a
+ * group's events are the concatenation of its images'.  The session records each column's draft base at encode time, from
+ * the group's reference (stage with _stage_device_draft).
+ * ---------------------------------------------------------------------- */
+#define PB_EDIT_COLUMN   0      /* a deletion, substitution or insertion column                                    */
+#define PB_EDIT_COVERAGE 1      /* position = first index-0 position the image won, index = last - first           */
+typedef struct {
+    int64_t position;
+    int32_t index;
+    uint8_t label;              /* network label 0..4 (0 = deleted, 1..4 = A, C, G, T)                             */
+    uint8_t phred;              /* the column's network phred                                                      */
+    uint8_t draft;              /* upper-cased draft base at `position`                                            */
+    uint8_t kind;               /* PB_EDIT_COLUMN or PB_EDIT_COVERAGE                                              */
+} pb_edit_event_t;
+/* attach an event sink [capacity_events] to the session begun last; call before the first stage */
+int pb_polish_stream_edits(pb_polish_encoder_t *enc, int64_t capacity_events, pb_edit_event_t *d_events);
+/* stage_device with the group's reference strings (d_ref, addressed by the regions' ref_off / ref_len): required in an edits
+ * session, and read by run() only                                                                                   */
+int pb_polish_stream_stage_device_draft(pb_polish_encoder_t *enc, const pb_reads_t *d_reads, const pb_region_t *h_regions,
+                                        int64_t g0, int64_t g1, int32_t region_id0, const char *d_ref);
+/* after _end: the events of the session (PB_ERR_CAPACITY from _end with *n_events > capacity_events: restart larger), and
+ * the events of each group in run order                                                                              */
+int pb_polish_stream_event_total(pb_polish_encoder_t *enc, int64_t *n_events);
+int pb_polish_stream_group_events(pb_polish_encoder_t *enc, int64_t *h_events, int64_t n_groups);
+/* diagnostics: pb_test_polish_stitch_sink (byte records in h_records) with the event sink of an edits session; h_phred
+ * and h_draft uint8 [n_images][1000]: each column's phred and upper-cased draft base.  PB_ERR_CAPACITY when either sink
+ * overflows.                                                                                                         */
+int pb_test_polish_stitch_sink_edits(const uint8_t *h_bases, const uint8_t *h_phred, const uint8_t *h_draft,
+                                     const int64_t *h_position, const int32_t *h_index, const int32_t *h_image_region,
+                                     const int32_t *h_chunk_id, const int64_t *h_region_starts, int64_t n_regions,
+                                     int64_t n_images, int64_t chunk, char *h_records, int64_t capacity, int64_t *n_out,
+                                     int64_t *h_region_records, pb_edit_event_t *h_events, int64_t capacity_events,
+                                     int64_t *n_events, int64_t *h_region_events, void *stream);
+/* The edits VCF records of one contig on the device.  d_events: the contig's PB_EDIT_COLUMN events, sorted by (position,
+ * index) (the group order of a session); h_cover [n_cover][2]: the inclusive position ranges its images won at index 0;
+ * the contig's polished span [span_start, span_end]; d_draft: the contig's draft bases [span_start, span_end] (any case).
+ * Writes the records' text lines (CHROM POS ID REF ALT QUAL FILTER INFO, '\n'-terminated, POS sorted) to d_text
+ * [capacity_text] and per line (0-based POS, REF length, text bytes) to d_lines [capacity_lines][3]; *n_lines / *n_text =
+ * lines and bytes needed (PB_ERR_CAPACITY when either exceeds its capacity).                                          */
+int pb_polish_edits_vcf_device(const pb_edit_event_t *d_events, int64_t n_events, const int64_t *h_cover, int64_t n_cover,
+                               int64_t span_start, int64_t span_end, const char *d_draft, const char *contig,
+                               char *d_text, int64_t capacity_text, int64_t *d_lines, int64_t capacity_lines,
+                               int64_t *n_lines, int64_t *n_text, void *stream);
+
+/* ------------------------------------------------------------------------
  * Candidate selection (SURVEY 8f row f2).  Replaces the per-candidate logic of
  * small_chunk_stitch, pepper_variant/modules/python/CandidateFinder.py:356-530:
  * homopolymer context of the +-10 bp reference window (:393-406), genotype =

@@ -61,8 +61,15 @@ struct SinkArgs {
     int64_t *state = nullptr;                                    // [0] running sink offset (records needed so far)
     int64_t *group_bytes = nullptr;                              // records per slot
     char *out = nullptr; int64_t capacity = 0;                   // capacity in records
+    // edits session (events set): the columns' phred and draft bases [n][1000] and the event sink; state[1] = events needed
+    // so far
+    const uint8_t *edit_phred = nullptr, *draft = nullptr;
+    pb_edit_event_t *events = nullptr; int64_t ev_capacity = 0;
+    int64_t *group_events = nullptr;                             // events per slot
+    int32_t *ev_counts = nullptr; const int64_t *ev_offsets = nullptr;   // scratch (set by polish_sink)
 };
-int polish_sink(SinkArgs A, DevBuf &counts, DevBuf &offsets, cudaStream_t st);
+// ev: two scratch buffers (event counts, event offsets), needed when A.events is set
+int polish_sink(SinkArgs A, DevBuf &counts, DevBuf &offsets, cudaStream_t st, DevBuf *ev = nullptr);
 struct PolishStream;       // streaming polish session state (pipeline.cu)
 void polish_stream_free(PolishStream *S);
 int tc_upload_rnn(TcRnn &T, const float *Wp, const float *bias, int K0, int K0p_src, int H, int Kp_src);

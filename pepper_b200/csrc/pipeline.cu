@@ -16,7 +16,9 @@ struct ChunkRow { int64_t col_start; int32_t nvalid; int32_t region; int32_t chu
 
 __global__ void k_polish_chunk(const ChunkRow *__restrict__ rows, const uint8_t *__restrict__ image, const int64_t *__restrict__ pos,
                                const int32_t *__restrict__ idx, uint8_t *__restrict__ imgs, int64_t *__restrict__ position,
-                               int32_t *__restrict__ index, int32_t *__restrict__ iregion, int32_t *__restrict__ cid) {
+                               int32_t *__restrict__ index, int32_t *__restrict__ iregion, int32_t *__restrict__ cid,
+                               uint8_t *__restrict__ draft = nullptr, const char *__restrict__ ref = nullptr,
+                               const pb_region_t *__restrict__ regions = nullptr, int32_t region0 = 0) {
     const int64_t k = blockIdx.x;
     const ChunkRow r = rows[k];
     for (int i = threadIdx.x; i < PB_POLISH_SEQ_LEN * PB_POLISH_FEATURES; i += blockDim.x) {
@@ -26,6 +28,16 @@ __global__ void k_polish_chunk(const ChunkRow *__restrict__ rows, const uint8_t 
     for (int c = threadIdx.x; c < PB_POLISH_SEQ_LEN; c += blockDim.x) {
         position[k * PB_POLISH_SEQ_LEN + c] = (c < r.nvalid) ? pos[r.col_start + c] : -1;
         index[k * PB_POLISH_SEQ_LEN + c] = (c < r.nvalid) ? idx[r.col_start + c] : -1;
+    }
+    // an edits session: each column's upper-cased draft base, from the region's reference string
+    if (draft) {
+        const pb_region_t rg = regions[r.region - region0];
+        for (int c = threadIdx.x; c < PB_POLISH_SEQ_LEN; c += blockDim.x) {
+            const int64_t o = (c < r.nvalid) ? pos[r.col_start + c] - rg.ref_start : -1;
+            char b = (o >= 0 && o < rg.ref_len) ? ref[rg.ref_off + o] : 0;
+            if (b >= 'a' && b <= 'z') b = (char) (b - 32);
+            draft[k * PB_POLISH_SEQ_LEN + c] = (uint8_t) b;
+        }
     }
     if (threadIdx.x == 0) { iregion[k] = r.region; cid[k] = r.chunk_id; }
 }
@@ -587,6 +599,8 @@ struct PolishStream {
     char *d_sink = nullptr;
     int64_t capacity = 0;                       // sink records
     bool qualities = false;                     // records are (base, QV byte) pairs
+    pb_edit_event_t *d_events = nullptr;        // edits session: the event sink (pb_polish_stream_edits)
+    int64_t ev_capacity = 0;
     GroupView V[2];
     int32_t region_id0[2] = {0, 0};
     bool staged[2] = {false, false};
@@ -596,8 +610,8 @@ struct PolishStream {
     int64_t pending = 0, ring_cap = 0;
     std::vector<int32_t> h_region, h_cid;       // host copy of the pending images' region id / chunk id
     int32_t prev_region = -1, prev_cid = 0;     // the last image that went through the network
-    DevBuf imgs, position, index, region, cid, start, slot;
-    DevBuf bases, phred, counts, offsets, state, group_bytes;
+    DevBuf imgs, position, index, region, cid, start, slot, draft;
+    DevBuf bases, phred, counts, offsets, state, group_bytes, group_events, ev_scratch[2];
     int64_t group_cap = 0;
     std::vector<cudaEvent_t> ev;                // per group: encoder start, encoder end, network (+ sink) end
     int64_t ev_done = 0;
@@ -607,8 +621,8 @@ struct PolishStream {
 
 void polish_stream_free(PolishStream *S) {
     if (!S) return;
-    DevBuf *bufs[] = {&S->imgs, &S->position, &S->index, &S->region, &S->cid, &S->start, &S->slot, &S->bases, &S->phred, &S->counts,
-                      &S->offsets, &S->state, &S->group_bytes};
+    DevBuf *bufs[] = {&S->imgs, &S->position, &S->index, &S->region, &S->cid, &S->start, &S->slot, &S->draft, &S->bases, &S->phred,
+                      &S->counts, &S->offsets, &S->state, &S->group_bytes, &S->group_events, &S->ev_scratch[0], &S->ev_scratch[1]};
     for (auto *b : bufs) b->release();
     for (auto x : S->ev) cudaEventDestroy(x);
     delete S;
@@ -627,11 +641,16 @@ static int grow_keep(DevBuf &b, size_t need, size_t keep, cudaStream_t st) {
     return PB_OK;
 }
 
-// bytes per pending image in each image buffer (images, position, index, region, chunk id, region start, group slot)
-static const size_t PS_BYTES[7] = {(size_t) PB_POLISH_SEQ_LEN * PB_POLISH_FEATURES, sizeof(int64_t) * PB_POLISH_SEQ_LEN,
-                                   sizeof(int32_t) * PB_POLISH_SEQ_LEN, sizeof(int32_t), sizeof(int32_t), sizeof(int64_t), sizeof(int32_t)};
-static void ps_buffers(PolishStream *S, DevBuf *B[7]) {
+// bytes per pending image in each image buffer (images, position, index, region, chunk id, region start, group slot, and in an
+// edits session the columns' draft bases)
+static const size_t PS_BYTES[8] = {(size_t) PB_POLISH_SEQ_LEN * PB_POLISH_FEATURES, sizeof(int64_t) * PB_POLISH_SEQ_LEN,
+                                   sizeof(int32_t) * PB_POLISH_SEQ_LEN, sizeof(int32_t), sizeof(int32_t), sizeof(int64_t), sizeof(int32_t),
+                                   (size_t) PB_POLISH_SEQ_LEN};
+// the image buffers of the session; returns how many are in use
+static int ps_buffers(PolishStream *S, DevBuf *B[8]) {
     B[0] = &S->imgs; B[1] = &S->position; B[2] = &S->index; B[3] = &S->region; B[4] = &S->cid; B[5] = &S->start; B[6] = &S->slot;
+    B[7] = &S->draft;
+    return S->d_events ? 8 : 7;
 }
 
 static int psession(pb_polish_encoder_t *e, PolishStream **S, bool need_active) {
@@ -654,13 +673,14 @@ static int polish_stream_begin(pb_polish_encoder_t *e, pb_polish_net_t *net, int
     PB_TRY(ensure_events(e->pevt, 3));
     S->st = (cudaStream_t) stream_;
     S->d_sink = d_sink; S->capacity = std::max<int64_t>(capacity, 0); S->qualities = qualities;
+    S->d_events = nullptr; S->ev_capacity = 0;
     S->staged[0] = S->staged[1] = false; S->next_stage = 0; S->next_run = 0;
     S->pending = 0; S->h_region.clear(); S->h_cid.clear(); S->prev_region = -1; S->prev_cid = 0;
     S->ev_done = 0; S->enc_ms = S->net_ms = 0.f;
     S->cols = S->images = S->net_launches = S->groups = 0;
-    PB_TRY(S->state.reserve(sizeof(int64_t)));
+    PB_TRY(S->state.reserve(2 * sizeof(int64_t)));
     if (S->group_cap == 0) { PB_TRY(S->group_bytes.reserve(sizeof(int64_t) * 256)); S->group_cap = 256; }
-    PB_CUDA(cudaMemsetAsync(S->state.p, 0, sizeof(int64_t), S->st));
+    PB_CUDA(cudaMemsetAsync(S->state.p, 0, 2 * sizeof(int64_t), S->st));
     PB_CUDA(cudaMemsetAsync(S->group_bytes.p, 0, sizeof(int64_t) * S->group_cap, S->st));
     S->active = true;
     return PB_OK;
@@ -676,11 +696,26 @@ extern "C" int pb_polish_stream_begin_qual(pb_polish_encoder_t *e, pb_polish_net
     return polish_stream_begin(e, net, capacity_records, d_sink, true, stream_);
 }
 
-// regions [g0, g1) of a workload resident in HBM: only the re-based region rows are copied (copy stream)
-extern "C" int pb_polish_stream_stage_device(pb_polish_encoder_t *e, const pb_reads_t *d_reads, const pb_region_t *h_regions,
-                                             int64_t g0, int64_t g1, int32_t region_id0) {
+// the event sink of an edits session: set after _begin, before the first group is staged
+extern "C" int pb_polish_stream_edits(pb_polish_encoder_t *e, int64_t capacity_events, pb_edit_event_t *d_events) {
     PolishStream *S;
     PB_TRY(psession(e, &S, true));
+    if (!d_events) { set_error("null argument"); return PB_ERR_ARG; }
+    if (S->groups > 0 || S->staged[0] || S->staged[1]) { set_error("the event sink is attached before the first stage"); return PB_ERR_STATE; }
+    S->d_events = d_events; S->ev_capacity = std::max<int64_t>(capacity_events, 0);
+    if (S->ring_cap > 0) PB_TRY(S->draft.reserve(PS_BYTES[7] * S->ring_cap));      // the ring may have grown in an earlier session
+    if (S->group_events.cap < sizeof(int64_t) * S->group_cap) PB_TRY(S->group_events.reserve(sizeof(int64_t) * S->group_cap));
+    PB_CUDA(cudaMemsetAsync(S->group_events.p, 0, sizeof(int64_t) * S->group_cap, S->st));
+    return PB_OK;
+}
+
+// regions [g0, g1) of a workload resident in HBM: only the re-based region rows are copied (copy stream).  d_ref: the group's
+// reference strings (an edits session reads each column's draft base from them when the group is run)
+static int polish_stream_stage(pb_polish_encoder_t *e, const pb_reads_t *d_reads, const pb_region_t *h_regions, int64_t g0, int64_t g1,
+                               int32_t region_id0, const char *d_ref) {
+    PolishStream *S;
+    PB_TRY(psession(e, &S, true));
+    if (S->d_events && !d_ref) { set_error("an edits session stages groups with their reference (_stage_device_draft)"); return PB_ERR_ARG; }
     if (!d_reads || !h_regions || g0 < 0 || g1 <= g0) { set_error("bad group [%lld, %lld)", (long long) g0, (long long) g1); return PB_ERR_ARG; }
     const int b = S->next_stage;
     if (S->staged[b]) { set_error("both staging buffers are in use: run a staged group first"); return PB_ERR_STATE; }
@@ -695,9 +730,20 @@ extern "C" int pb_polish_stream_stage_device(pb_polish_encoder_t *e, const pb_re
     V.d.n_reads = r1 - r0;
     V.d.pos += r0; V.d.seq_off += r0; V.d.cigar_off += r0; V.d.flags += r0; V.d.mapq += r0;     // seq / qual / cigar keep absolute offsets
     V.d_regions = e->g_regions[b].as<pb_region_t>();
-    V.d_ref = nullptr;
+    V.d_ref = d_ref;
     S->staged[b] = true; S->region_id0[b] = region_id0; S->next_stage = b ^ 1;
     return PB_OK;
+}
+
+extern "C" int pb_polish_stream_stage_device(pb_polish_encoder_t *e, const pb_reads_t *d_reads, const pb_region_t *h_regions,
+                                             int64_t g0, int64_t g1, int32_t region_id0) {
+    return polish_stream_stage(e, d_reads, h_regions, g0, g1, region_id0, nullptr);
+}
+
+extern "C" int pb_polish_stream_stage_device_draft(pb_polish_encoder_t *e, const pb_reads_t *d_reads, const pb_region_t *h_regions,
+                                                   int64_t g0, int64_t g1, int32_t region_id0, const char *d_ref) {
+    if (!d_ref) { set_error("null reference"); return PB_ERR_ARG; }
+    return polish_stream_stage(e, d_reads, h_regions, g0, g1, region_id0, d_ref);
 }
 
 // the network + stitch-to-sink over every whole chunk of the pending images (`flush`: over all of them), then the images left
@@ -725,16 +771,20 @@ static int polish_stream_network(pb_polish_net_t *net, PolishStream *S, bool flu
         A.prev_region = done > 0 ? S->h_region[done - 1] : S->prev_region;
         A.prev_cid = done > 0 ? S->h_cid[done - 1] : S->prev_cid;
         A.state = S->state.as<int64_t>(); A.group_bytes = S->group_bytes.as<int64_t>(); A.out = S->d_sink; A.capacity = S->capacity;
-        PB_TRY(polish_sink(A, S->counts, S->offsets, st));
+        if (S->d_events) {
+            A.edit_phred = S->phred.as<uint8_t>(); A.draft = S->draft.as<uint8_t>() + done * PB_POLISH_SEQ_LEN;
+            A.events = S->d_events; A.ev_capacity = S->ev_capacity; A.group_events = S->group_events.as<int64_t>();
+        }
+        PB_TRY(polish_sink(A, S->counts, S->offsets, st, S->ev_scratch));
         done += B;
     }
     if (done == 0) return PB_OK;
     S->prev_region = S->h_region[done - 1]; S->prev_cid = S->h_cid[done - 1];
     const int64_t tail = S->pending - done;          // < one chunk <= done: source and destination do not overlap
-    DevBuf *Bf[7];
-    ps_buffers(S, Bf);
+    DevBuf *Bf[8];
+    const int nb = ps_buffers(S, Bf);
     if (tail > 0)
-        for (int k = 0; k < 7; k++)
+        for (int k = 0; k < nb; k++)
             PB_CUDA(cudaMemcpyAsync(Bf[k]->p, Bf[k]->as<char>() + done * PS_BYTES[k], tail * PS_BYTES[k], cudaMemcpyDeviceToDevice, st));
     S->h_region.erase(S->h_region.begin(), S->h_region.begin() + done);
     S->h_cid.erase(S->h_cid.begin(), S->h_cid.begin() + done);
@@ -768,13 +818,17 @@ extern "C" int pb_polish_stream_run(pb_polish_encoder_t *e, pb_polish_net_t *net
         const int64_t cap = 2 * S->group_cap;
         PB_TRY(grow_keep(S->group_bytes, sizeof(int64_t) * cap, sizeof(int64_t) * S->group_cap, st));
         PB_CUDA(cudaMemsetAsync(S->group_bytes.as<int64_t>() + S->group_cap, 0, sizeof(int64_t) * (cap - S->group_cap), st));
+        if (S->d_events) {
+            PB_TRY(grow_keep(S->group_events, sizeof(int64_t) * cap, sizeof(int64_t) * S->group_cap, st));
+            PB_CUDA(cudaMemsetAsync(S->group_events.as<int64_t>() + S->group_cap, 0, sizeof(int64_t) * (cap - S->group_cap), st));
+        }
         S->group_cap = cap;
     }
     if (p0 + n_new > S->ring_cap) {
-        DevBuf *Bf[7];
-        ps_buffers(S, Bf);
+        DevBuf *Bf[8];
+        const int nb = ps_buffers(S, Bf);
         const int64_t cap = std::max<int64_t>(p0 + n_new, POLISH_NET_CHUNK);
-        for (int k = 0; k < 7; k++) PB_TRY(grow_keep(*Bf[k], PS_BYTES[k] * cap, PS_BYTES[k] * p0, st));
+        for (int k = 0; k < nb; k++) PB_TRY(grow_keep(*Bf[k], PS_BYTES[k] * cap, PS_BYTES[k] * p0, st));
         S->ring_cap = cap;
     }
     if (n_new > 0) {
@@ -789,7 +843,9 @@ extern "C" int pb_polish_stream_run(pb_polish_encoder_t *e, pb_polish_net_t *net
                                                          e->p_idx.as<int32_t>(), S->imgs.as<uint8_t>() + p0 * PS_BYTES[0],
                                                          S->position.as<int64_t>() + p0 * PB_POLISH_SEQ_LEN,
                                                          S->index.as<int32_t>() + p0 * PB_POLISH_SEQ_LEN, S->region.as<int32_t>() + p0,
-                                                         S->cid.as<int32_t>() + p0);
+                                                         S->cid.as<int32_t>() + p0,
+                                                         S->d_events ? S->draft.as<uint8_t>() + p0 * PB_POLISH_SEQ_LEN : nullptr,
+                                                         V.d_ref, V.d_regions, region0);
         PB_CUDA(cudaGetLastError());
         PB_CUDA(cudaMemcpyAsync(S->start.as<int64_t>() + p0, h_start.data(), sizeof(int64_t) * n_new, cudaMemcpyHostToDevice, st));
         PB_CUDA(cudaMemcpyAsync(S->slot.as<int32_t>() + p0, h_slot.data(), sizeof(int32_t) * n_new, cudaMemcpyHostToDevice, st));
@@ -842,6 +898,35 @@ extern "C" int pb_polish_stream_end(pb_polish_encoder_t *e, pb_polish_net_t *net
         set_error("consensus sink capacity %lld < %lld bytes needed", (long long) S->capacity, (long long) total);
         return PB_ERR_CAPACITY;
     }
+    if (S->d_events) {
+        int64_t n_ev = 0;
+        PB_TRY(pb_polish_stream_event_total(e, &n_ev));
+        if (n_ev > S->ev_capacity) {
+            set_error("edit event sink capacity %lld < %lld events needed", (long long) S->ev_capacity, (long long) n_ev);
+            return PB_ERR_CAPACITY;
+        }
+    }
+    return PB_OK;
+}
+
+// events needed by the last edits session so far (all of them after _end)
+extern "C" int pb_polish_stream_event_total(pb_polish_encoder_t *e, int64_t *n_events) {
+    if (!e || !e->pstream || !e->pstream->d_events) { set_error("no edits session"); return PB_ERR_STATE; }
+    if (!n_events) { set_error("null argument"); return PB_ERR_ARG; }
+    PolishStream *S = e->pstream;
+    PB_CUDA(cudaMemcpyAsync(n_events, S->state.as<int64_t>() + 1, sizeof(int64_t), cudaMemcpyDeviceToHost, S->st));
+    PB_CUDA(cudaStreamSynchronize(S->st));
+    return PB_OK;
+}
+
+// events of each group of the last edits session, in the order the groups were run (call after _end)
+extern "C" int pb_polish_stream_group_events(pb_polish_encoder_t *e, int64_t *h_events, int64_t n_groups) {
+    if (!e || !e->pstream || !e->pstream->d_events) { set_error("no edits session"); return PB_ERR_STATE; }
+    PolishStream *S = e->pstream;
+    if (!h_events || n_groups < 0 || n_groups > S->groups) { set_error("bad argument"); return PB_ERR_ARG; }
+    if (n_groups == 0) return PB_OK;
+    PB_CUDA(cudaMemcpyAsync(h_events, S->group_events.p, sizeof(int64_t) * n_groups, cudaMemcpyDeviceToHost, S->st));
+    PB_CUDA(cudaStreamSynchronize(S->st));
     return PB_OK;
 }
 

@@ -93,6 +93,73 @@ __global__ void __launch_bounds__(256) k_stitch(const uint8_t *__restrict__ base
     if (!WRITE && threadIdx.x == 0) counts[im] = total;
 }
 
+// The edit events of one image of an edits session (pb_edit_event_t), written in order from event o0 when WRITE (o < ev_capacity).
+// A column wins its (position, index) by the rule of stitch_columns with label-0 columns kept; a winner is an event when it
+// is a deletion (label 0 at index 0), a substitution (label != draft base at index 0) or an insertion (index >= 1, label !=
+// 0).  After the columns, one PB_EDIT_COVERAGE record: the first and last index-0 position the image won (none: no record).
+// Returns the records.
+template <bool WRITE>
+__device__ int edit_columns(const SinkArgs &A, int64_t im, bool tail_lost, bool head_lost, int64_t o0) {
+    __shared__ int s_warp[8];
+    __shared__ int s_carry;
+    __shared__ unsigned long long s_first, s_last;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint8_t *bases = A.bases + im * SCOLS, *phred = A.edit_phred + im * SCOLS, *draft = A.draft + im * SCOLS;
+    const int64_t *position = A.position + im * SCOLS;
+    const int32_t *index = A.index + im * SCOLS;
+    const int64_t st = A.start[im];
+    if (tid == 0) { s_carry = 0; s_first = ~0ull; s_last = 0ull; }
+    __syncthreads();
+    bool won0 = false;
+    for (int c0 = 0; c0 < SCOLS; c0 += 256) {
+        const int c = c0 + tid;
+        bool ev = false;
+        uint8_t b = 0;
+        int64_t pos = -1;
+        int idx = -1;
+        if (c < SCOLS) {
+            pos = position[c];
+            idx = index[c];
+            b = bases[c];
+            bool win = pos >= 0 && idx >= 0 && !(st > 0 && pos <= st + S_BUFFER) && b <= 4;
+            if (tail_lost && c >= SCOLS - S_OVERLAP) win = false;
+            if (head_lost && c < S_OVERLAP) win = false;
+            if (win && idx == 0) {
+                won0 = true;
+                atomicMin(&s_first, (unsigned long long) pos);
+                atomicMax(&s_last, (unsigned long long) pos);
+            }
+            ev = win && (idx == 0 ? (b == 0 || (uint8_t) "ACGT"[b - 1] != draft[c]) : b != 0);
+        }
+        const unsigned m = __ballot_sync(0xffffffffu, ev);
+        const int wcount = __popc(m), wprefix = __popc(m & ((1u << lane) - 1u));
+        if (lane == 0) s_warp[warp] = wcount;
+        __syncthreads();
+        int base = s_carry;
+        for (int w = 0; w < warp; w++) base += s_warp[w];
+        if (WRITE && ev) {
+            const int64_t o = o0 + base + wprefix;
+            if (o < A.ev_capacity) {
+                pb_edit_event_t e;
+                e.position = pos; e.index = idx; e.label = b; e.phred = phred[c]; e.draft = draft[c]; e.kind = PB_EDIT_COLUMN;
+                A.events[o] = e;
+            }
+        }
+        __syncthreads();
+        if (tid == 0) { int s = 0; for (int w = 0; w < 8; w++) s += s_warp[w]; s_carry += s; }
+        __syncthreads();
+    }
+    const bool covered = __syncthreads_or(won0);
+    const int total = s_carry;
+    if (WRITE && covered && tid == 0 && o0 + total < A.ev_capacity) {
+        pb_edit_event_t e;
+        e.position = (int64_t) s_first; e.index = (int32_t) (s_last - s_first); e.label = 0; e.phred = 0; e.draft = 0;
+        e.kind = PB_EDIT_COVERAGE;
+        A.events[o0 + total] = e;
+    }
+    return total + (covered ? 1 : 0);
+}
+
 // Stitch-to-sink: the same rule over one network chunk of a streaming polish session, appended to a sink at a running record
 // offset that stays on the device.  A record is one consensus byte, or with A.phred the 2 bytes (base, QV byte).  The
 // neighbours that decide the overlaps may lie outside the chunk: the next image's region / chunk id come from the session's
@@ -114,21 +181,37 @@ __global__ void __launch_bounds__(256) k_stitch_sink(SinkArgs A) {
         A.counts[im] = total;
         if (total) atomicAdd(reinterpret_cast<unsigned long long *>(A.group_bytes + A.slot[im]), (unsigned long long) total);
     }
+    if (A.events) {
+        const int ne = edit_columns<WRITE>(A, im, tail_lost, head_lost, WRITE ? A.state[1] + A.ev_offsets[im] : 0);
+        if (!WRITE && threadIdx.x == 0) {
+            A.ev_counts[im] = ne;
+            if (ne) atomicAdd(reinterpret_cast<unsigned long long *>(A.group_events + A.slot[im]), (unsigned long long) ne);
+        }
+    }
 }
 
 __global__ void k_sink_advance(int64_t *state, const int64_t *chunk_total) { state[0] += *chunk_total; }
 
 // count, scan, write, advance: four launches on `st`, no host synchronisation
-int polish_sink(SinkArgs A, DevBuf &counts, DevBuf &offsets, cudaStream_t st) {
+int polish_sink(SinkArgs A, DevBuf &counts, DevBuf &offsets, cudaStream_t st, DevBuf *ev) {
     if (A.n <= 0) return PB_OK;
     PB_TRY(counts.reserve(sizeof(int32_t) * A.n));
     PB_TRY(offsets.reserve(sizeof(int64_t) * (A.n + 1)));
     A.counts = counts.as<int32_t>();
     A.offsets = offsets.as<int64_t>();
+    if (A.events) {
+        if (!ev) { set_error("edits sink without scratch"); return PB_ERR_ARG; }
+        PB_TRY(ev[0].reserve(sizeof(int32_t) * A.n));
+        PB_TRY(ev[1].reserve(sizeof(int64_t) * (A.n + 1)));
+        A.ev_counts = ev[0].as<int32_t>();
+        A.ev_offsets = ev[1].as<int64_t>();
+    }
     k_stitch_sink<false><<<(unsigned) A.n, 256, 0, st>>>(A);
     k_scan_excl<<<1, 1024, 0, st>>>(A.counts, offsets.as<int64_t>(), A.n, nullptr);
+    if (A.events) k_scan_excl<<<1, 1024, 0, st>>>(A.ev_counts, ev[1].as<int64_t>(), A.n, nullptr);
     k_stitch_sink<true><<<(unsigned) A.n, 256, 0, st>>>(A);
     k_sink_advance<<<1, 1, 0, st>>>(A.state, offsets.as<int64_t>() + A.n);
+    if (A.events) k_sink_advance<<<1, 1, 0, st>>>(A.state + 1, ev[1].as<int64_t>() + A.n);
     PB_CUDA(cudaGetLastError());
     return PB_OK;
 }
@@ -236,12 +319,20 @@ extern "C" int pb_polish_stitch_qual_host(const uint8_t *h_bases, const uint8_t 
 
 // diagnostics: host predictions (images in session order) through the stitch-to-sink kernel `chunk` images at a time, the way a
 // streaming session feeds it one network chunk after the other.  h_region_bytes (optional): records per region [n_regions].
-// Given h_phred, h_out holds 2-byte (base, QV byte) records [capacity].
+// Given h_phred, h_out holds 2-byte (base, QV byte) records [capacity].  Given h_draft (and h_ev_phred), the event sink of an
+// edits session: h_events [ev_capacity], *n_events, h_region_events (optional) [n_regions].
+struct EditTest {
+    const uint8_t *h_phred = nullptr, *h_draft = nullptr;
+    pb_edit_event_t *h_events = nullptr; int64_t capacity = 0; int64_t *n_events = nullptr, *h_region_events = nullptr;
+};
 static int stitch_sink_test(const uint8_t *h_bases, const uint8_t *h_phred, const int64_t *h_position, const int32_t *h_index,
                             const int32_t *h_image_region, const int32_t *h_chunk_id, const int64_t *h_region_starts,
                             int64_t n_regions, int64_t n_images, int64_t chunk, char *h_out, int64_t capacity,
-                            int64_t *n_out, int64_t *h_region_bytes, cudaStream_t st) {
+                            int64_t *n_out, int64_t *h_region_bytes, cudaStream_t st, const EditTest &E = EditTest()) {
+    const bool edits = E.h_draft != nullptr;
     if (!n_out || chunk <= 0 || n_regions <= 0) { set_error("bad argument"); return PB_ERR_ARG; }
+    if (edits && (!E.h_phred || !E.n_events || (E.capacity > 0 && !E.h_events))) { set_error("null argument"); return PB_ERR_ARG; }
+    if (edits) *E.n_events = 0;
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev < 1) { set_error("no CUDA device: libpepper_b200 has no CPU fallback"); return PB_ERR_CUDA; }
     *n_out = 0;
@@ -252,7 +343,7 @@ static int stitch_sink_test(const uint8_t *h_bases, const uint8_t *h_phred, cons
         if (h_image_region[i] < 0 || h_image_region[i] >= n_regions) { set_error("image %lld: region out of range", (long long) i); return PB_ERR_ARG; }
         start[i] = h_region_starts[h_image_region[i]];
     }
-    DevBuf b, ph, p, i, r, c, s, o, state, gb, counts, offsets;
+    DevBuf b, ph, p, i, r, c, s, o, state, gb, counts, offsets, eph, dr, evo, ge, evs[2];
     int rc = PB_OK;
     do {
         if ((rc = upload(b, h_bases, (size_t) n_images * SCOLS, st)) != PB_OK) break;
@@ -263,9 +354,16 @@ static int stitch_sink_test(const uint8_t *h_bases, const uint8_t *h_phred, cons
         if ((rc = upload(c, h_chunk_id, sizeof(int32_t) * n_images, st)) != PB_OK) break;
         if ((rc = upload(s, start.data(), sizeof(int64_t) * n_images, st)) != PB_OK) break;
         if ((rc = o.reserve(rec * (size_t) std::max<int64_t>(capacity, 1))) != PB_OK) break;
-        if ((rc = state.reserve(sizeof(int64_t))) != PB_OK) break;
+        if ((rc = state.reserve(2 * sizeof(int64_t))) != PB_OK) break;
         if ((rc = gb.reserve(sizeof(int64_t) * n_regions)) != PB_OK) break;
-        if (cudaMemsetAsync(state.p, 0, sizeof(int64_t), st) != cudaSuccess || cudaMemsetAsync(gb.p, 0, sizeof(int64_t) * n_regions, st) != cudaSuccess) {
+        if (edits) {
+            if ((rc = upload(eph, E.h_phred, (size_t) n_images * SCOLS, st)) != PB_OK) break;
+            if ((rc = upload(dr, E.h_draft, (size_t) n_images * SCOLS, st)) != PB_OK) break;
+            if ((rc = evo.reserve(sizeof(pb_edit_event_t) * (size_t) std::max<int64_t>(E.capacity, 1))) != PB_OK) break;
+            if ((rc = ge.reserve(sizeof(int64_t) * n_regions)) != PB_OK) break;
+            if (cudaMemsetAsync(ge.p, 0, sizeof(int64_t) * n_regions, st) != cudaSuccess) { set_error("memset failed"); rc = PB_ERR_CUDA; break; }
+        }
+        if (cudaMemsetAsync(state.p, 0, 2 * sizeof(int64_t), st) != cudaSuccess || cudaMemsetAsync(gb.p, 0, sizeof(int64_t) * n_regions, st) != cudaSuccess) {
             set_error("memset failed"); rc = PB_ERR_CUDA; break;
         }
         for (int64_t c0 = 0; c0 < n_images && rc == PB_OK; c0 += chunk) {
@@ -276,7 +374,11 @@ static int stitch_sink_test(const uint8_t *h_bases, const uint8_t *h_phred, cons
             A.region = r.as<int32_t>() + c0; A.cid = c.as<int32_t>() + c0; A.start = s.as<int64_t>() + c0; A.slot = r.as<int32_t>() + c0;
             A.prev_region = c0 > 0 ? h_image_region[c0 - 1] : -1; A.prev_cid = c0 > 0 ? h_chunk_id[c0 - 1] : 0;
             A.state = state.as<int64_t>(); A.group_bytes = gb.as<int64_t>(); A.out = o.as<char>(); A.capacity = capacity;
-            rc = polish_sink(A, counts, offsets, st);
+            if (edits) {
+                A.edit_phred = eph.as<uint8_t>() + c0 * SCOLS; A.draft = dr.as<uint8_t>() + c0 * SCOLS;
+                A.events = evo.as<pb_edit_event_t>(); A.ev_capacity = E.capacity; A.group_events = ge.as<int64_t>();
+            }
+            rc = polish_sink(A, counts, offsets, st, evs);
         }
         if (rc != PB_OK) break;
         int64_t total = 0;
@@ -285,14 +387,22 @@ static int stitch_sink_test(const uint8_t *h_bases, const uint8_t *h_phred, cons
         if (e == cudaSuccess) e = cudaStreamSynchronize(st);
         if (e != cudaSuccess) { set_error("stitch sink: %s", cudaGetErrorString(e)); rc = PB_ERR_CUDA; break; }
         *n_out = total;
-        if (total > capacity) { set_error("consensus capacity %lld < %lld needed", (long long) capacity, (long long) total); rc = PB_ERR_CAPACITY; break; }
-        if (total > 0) {
-            e = cudaMemcpyAsync(h_out, o.p, rec * (size_t) total, cudaMemcpyDeviceToHost, st);
+        int64_t n_ev = 0;
+        if (edits) {
+            e = cudaMemcpyAsync(&n_ev, state.as<int64_t>() + 1, sizeof(int64_t), cudaMemcpyDeviceToHost, st);
+            if (e == cudaSuccess && E.h_region_events) e = cudaMemcpyAsync(E.h_region_events, ge.p, sizeof(int64_t) * n_regions, cudaMemcpyDeviceToHost, st);
             if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-            if (e != cudaSuccess) { set_error("stitch sink copy back: %s", cudaGetErrorString(e)); rc = PB_ERR_CUDA; }
+            if (e != cudaSuccess) { set_error("stitch sink: %s", cudaGetErrorString(e)); rc = PB_ERR_CUDA; break; }
+            *E.n_events = n_ev;
         }
+        if (total > capacity) { set_error("consensus capacity %lld < %lld needed", (long long) capacity, (long long) total); rc = PB_ERR_CAPACITY; break; }
+        if (n_ev > E.capacity) { set_error("edit event capacity %lld < %lld needed", (long long) E.capacity, (long long) n_ev); rc = PB_ERR_CAPACITY; break; }
+        if (total > 0) e = cudaMemcpyAsync(h_out, o.p, rec * (size_t) total, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess && n_ev > 0) e = cudaMemcpyAsync(E.h_events, evo.p, sizeof(pb_edit_event_t) * (size_t) n_ev, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) { set_error("stitch sink copy back: %s", cudaGetErrorString(e)); rc = PB_ERR_CUDA; }
     } while (0);
-    DevBuf *bufs[] = {&b, &ph, &p, &i, &r, &c, &s, &o, &state, &gb, &counts, &offsets};
+    DevBuf *bufs[] = {&b, &ph, &p, &i, &r, &c, &s, &o, &state, &gb, &counts, &offsets, &eph, &dr, &evo, &ge, &evs[0], &evs[1]};
     for (auto *x : bufs) x->release();
     return rc;
 }
@@ -313,4 +423,18 @@ extern "C" int pb_test_polish_stitch_sink_qual(const uint8_t *h_bases, const uin
     if (!h_phred) { set_error("null argument"); return PB_ERR_ARG; }
     return stitch_sink_test(h_bases, h_phred, h_position, h_index, h_image_region, h_chunk_id, h_region_starts, n_regions, n_images, chunk,
                             h_records, capacity, n_out, h_region_records, (cudaStream_t) stream_);
+}
+
+extern "C" int pb_test_polish_stitch_sink_edits(const uint8_t *h_bases, const uint8_t *h_phred, const uint8_t *h_draft,
+                                                const int64_t *h_position, const int32_t *h_index, const int32_t *h_image_region,
+                                                const int32_t *h_chunk_id, const int64_t *h_region_starts, int64_t n_regions,
+                                                int64_t n_images, int64_t chunk, char *h_records, int64_t capacity, int64_t *n_out,
+                                                int64_t *h_region_records, pb_edit_event_t *h_events, int64_t capacity_events,
+                                                int64_t *n_events, int64_t *h_region_events, void *stream_) {
+    if (!h_draft || !h_phred) { set_error("null argument"); return PB_ERR_ARG; }
+    EditTest E;
+    E.h_phred = h_phred; E.h_draft = h_draft; E.h_events = h_events; E.capacity = capacity_events; E.n_events = n_events;
+    E.h_region_events = h_region_events;
+    return stitch_sink_test(h_bases, nullptr, h_position, h_index, h_image_region, h_chunk_id, h_region_starts, n_regions, n_images, chunk,
+                            h_records, capacity, n_out, h_region_records, (cudaStream_t) stream_, E);
 }

@@ -492,16 +492,29 @@ class DistributedPolisher(_RankDriver):
 
     `qualities=True`: the session writes 2-byte polish.QUAL_RECORD records (base, FASTQ quality byte) in place of bytes, still
     gathered by one all-gather; `capacity_bytes` then counts records (consensus bases) and assemble() returns
-    {contig: (sequence, quality string)}."""
+    {contig: (sequence, quality string)}.
+
+    `edits=True`: the session also writes its edit events (polish_edits.EDIT_EVENT) into this rank's slice of a second, sparse
+    gather buffer of `capacity_events` events, gathered by group like the consensus; `write_edits(source, path)` then writes
+    the edits VCF.  A rank whose events overflow makes run() fail on every rank (PB_ERR_CAPACITY, `need_events` set)."""
 
     _claim_prefix = "pb_polish_claim"
 
     def __init__(self, state: dict, device: int, capacity_bytes: int, schedule: str = "dynamic", group_regions: int = 32,
-                 distributed: bool = True, caller=None, qualities: bool = False):
+                 distributed: bool = True, caller=None, qualities: bool = False, edits: bool = False, capacity_events: int = 0):
         from .pipeline import PolishCaller
         super().__init__(PolishCaller, state, device, schedule, group_regions, distributed, caller)
         self.capacity = int(capacity_bytes)
         self.qualities = bool(qualities)
+        self.edits = bool(edits)
+        self.capacity_events = int(capacity_events)
+        self.edits_buffer = None
+
+    def close(self):
+        if self.edits_buffer is not None:
+            self.edits_buffer.release()
+            self.edits_buffer = None
+        super().close()
 
     def run(self, source) -> int:
         """Returns this rank's consensus bytes (records with qualities); the gathered records of every rank are in self.buffer
@@ -511,12 +524,81 @@ class DistributedPolisher(_RankDriver):
         n_job = len(groups)
         self._gather_buffer(self.capacity, n_job, QUAL_RECORD if self.qualities else np.uint8)
         claimer = self._claimer(n_job, source.group_work(groups))
-        s = self.caller.stream(self.capacity, self.buffer.my_ptr(), qualities=self.qualities)
+        d_events = 0
+        if self.edits:
+            from .polish_edits import EDIT_EVENT
+            eb = self.edits_buffer
+            if eb is None or eb.max_groups < n_job or eb.capacity != self.capacity_events:
+                if eb is not None:
+                    eb.release()
+                self.edits_buffer = GatherBuffer(self.capacity_events, self.world, self.rank, self.device, max_groups=n_job,
+                                                 record=EDIT_EVENT)
+            d_events = self.edits_buffer.my_ptr()
+        s = self.caller.stream(self.capacity, self.buffer.my_ptr(), qualities=self.qualities, edits=self.edits,
+                               capacity_events=self.capacity_events, d_events=d_events)
+        from ._lib import PepperB200Error
         segments = self._run_job(s, claimer, groups, self.capacity, source)
-        n = s.end()
+        need_events = 0
+        try:
+            n = s.end()
+        except PepperB200Error as ex:
+            if not hasattr(ex, "need_events"):
+                raise
+            # the other ranks still gather: this rank joins with the events that fit, and every rank fails after the gather
+            n, need_events = ex.need, ex.need_events
         segments = [(g, int(k)) for (g, _), k in zip(segments, s.group_bytes())]
         self._gather(s, n, segments, n_job, "the consensus capacity (%d bytes per rank)" % self.capacity, "capacity_bytes")
+        if self.edits:
+            self._gather_events(s, segments, need_events)
         return n
+
+    def _gather_events(self, s, segments: list[tuple[int, int]], need: int):
+        """The events of every rank into edits_buffer, ordered by group like the consensus; fails on every rank when one rank's
+        events did not fit."""
+        import torch
+        from ._lib import PepperB200Error
+        from .abi import PB_ERR_CAPACITY
+        ev_seg = [(g, int(k)) for (g, _), k in zip(segments, s.group_events())]
+        ok = need == 0
+        self.edits_buffer.gather(sum(k for _, k in ev_seg) if ok else 0, ev_seg if ok else [])
+        worst = torch.tensor([need], dtype=torch.int64, device=self.device)
+        if self.world > 1:
+            import torch.distributed as dist
+            dist.all_reduce(worst, op=dist.ReduceOp.MAX)
+        need = int(worst.item())
+        if need:
+            ex = PepperB200Error("edit events overflow: %d events needed on one rank, capacity %d — raise `capacity_events`"
+                                 % (need, self.capacity_events), PB_ERR_CAPACITY)
+            ex.need_events = need
+            raise ex
+
+    def write_edits(self, source, path: str) -> None:
+        """The edits VCF of the last run (polish_edits.write_edits_vcf) at `path`, with its index: the gathered events cut at the
+        contig boundaries of the plan, turned into lines on the device contig by contig in the order of the polished FASTA, and
+        compressed there.  Contigs whose consensus is empty are left out, as the FASTA leaves them out."""
+        import torch
+        from .frontend import natural_key
+        from .polish_edits import events_by_contig, split_events, edits_vcf_device, device_part, write_edits_vcf
+        groups = source.groups(self.group_regions)
+        group_contig = [source.names[source.contig_of[g0]] for g0, _ in groups]
+        seq_len = {c: 0 for c in source.names}
+        for g, k in self.buffer.segments():
+            seq_len[group_contig[g]] += k
+        events = events_by_contig(self.edits_buffer.to_host(), self.edits_buffer.segments(), group_contig, source.names)
+        first = dict(zip(source.names, source._first[:-1]))
+        last = dict(zip(source.names, source._first[1:]))
+        dev = torch.device("cuda", self.device.index)
+        parts = []
+        for c in sorted(source.names, key=natural_key):
+            if not seq_len[c]:
+                continue
+            span = (source.intervals[first[c]][0], source.intervals[last[c] - 1][1])
+            columns, cover = split_events(events[c])
+            d_cols = torch.from_numpy(columns.view(np.uint8).reshape(-1)).to(dev)
+            d_draft = torch.from_numpy(source.fasta.fetch_array(c, span[0], span[1] + 1)).to(dev)
+            text, lines = edits_vcf_device(d_cols, cover, span, d_draft, c, self.device.index)
+            parts.append(device_part(c, text, lines, self.device.index))
+        write_edits_vcf(path, source.fasta_contigs(), parts)
 
     def assemble(self, source) -> dict:
         """{contig: polished sequence} of every contig of the source's plan (empty string: nothing survived), on every rank:

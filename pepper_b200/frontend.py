@@ -587,28 +587,39 @@ class PolishFromFiles(_FromFiles):
         return (seq, allc, regs) if return_calls else seq
 
     def polish_assembly(self, out_path: str | None = None, contigs: list[str] | None = None, group_regions: int = 32,
-                        capacity_bytes: int | None = None, realign: bool = True, fastq: bool = False) -> dict:
+                        capacity_bytes: int | None = None, realign: bool = True, fastq: bool = False, vcf_path: str | None = None,
+                        capacity_events: int | None = None) -> dict:
         """`pepper polish` of a whole assembly on this GPU: every contig common to the BAM and the FASTA (or `contigs`),
         make_images + call_consensus + the stitch on the device through one streaming session (dist.DistributedPolisher at world
         size 1).  Returns {contig: polished sequence} and, given `out_path`, writes the FASTA perform_stitch writes.
         `fastq`: the quality of every base is carried through the stitch; returns {contig: (sequence, quality string)} and
-        writes FASTQ (write_polished_fastq) to `out_path`."""
+        writes FASTQ (write_polished_fastq) to `out_path`.
+        `vcf_path`: also writes the edits VCF there (bgzipped, with its .tbi or .csi; polish_edits): a record for every run of
+        draft bases the stitch substituted, deleted or inserted after, with the least network phred of its columns as QUAL.
+        The return value is the same.  `capacity_events`: the first size of the event sink (doubled until it fits)."""
         from .dist import DistributedPolisher
         src = PolishFileSource(self.bam.path, self.fasta_path, contigs, self.device, self.threads, self.gpu_inflate, realign,
                                host_share=self.host_share)
         try:
-            cap = capacity_bytes or 2 * sum(e - s + 1 for s, e in src.intervals) + (1 << 20)
+            span = sum(e - s + 1 for s, e in src.intervals)
+            cap = capacity_bytes or 2 * span + (1 << 20)
+            ecap = capacity_events or span // 32 + (1 << 16)
             while True:
                 dp = DistributedPolisher(None, self.device, cap, "static", group_regions, distributed=False, caller=self.caller,
-                                         qualities=fastq)
+                                         qualities=fastq, edits=vcf_path is not None, capacity_events=ecap)
                 try:
                     dp.run(src)
                     seqs = dp.assemble(src)
+                    if vcf_path is not None:
+                        dp.write_edits(src, vcf_path)
                     break
-                except PepperB200Error as ex:        # consensus larger than the sink: restart the session larger
+                except PepperB200Error as ex:        # consensus or events larger than their sink: restart the session larger
                     if ex.rc != PB_ERR_CAPACITY:
                         raise
-                    cap *= 2
+                    if hasattr(ex, "need_events"):
+                        ecap *= 2
+                    else:
+                        cap *= 2
                 finally:
                     dp.close()
         finally:

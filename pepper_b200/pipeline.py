@@ -86,6 +86,10 @@ def _bind_calls(L):
     L.pb_polish_stream_end.argtypes = [vp, vp, C.POINTER(C.c_int64)]
     L.pb_polish_stream_stats.argtypes = [vp, vp, vp]
     L.pb_polish_stream_group_bytes.argtypes = [vp, vp, C.c_int64]
+    L.pb_polish_stream_edits.argtypes = [vp, C.c_int64, vp]
+    L.pb_polish_stream_stage_device_draft.argtypes = [vp, C.POINTER(PbReads), C.POINTER(PbRegion), C.c_int64, C.c_int64, C.c_int32, vp]
+    L.pb_polish_stream_event_total.argtypes = [vp, C.POINTER(C.c_int64)]
+    L.pb_polish_stream_group_events.argtypes = [vp, vp, C.c_int64]
     L._calls_bound = True
 
 
@@ -339,9 +343,10 @@ class PolishCaller:
         return d
 
 
-    def stream(self, capacity_bytes: int, d_sink: int, stream: int = 0, qualities: bool = False) -> "PolishStream":
+    def stream(self, capacity_bytes: int, d_sink: int, stream: int = 0, qualities: bool = False, edits: bool = False,
+               capacity_events: int = 0, d_events: int = 0) -> "PolishStream":
         """Streaming session over region groups with the stitch on the device (pb_polish_stream_*): see PolishStream."""
-        return PolishStream(self, capacity_bytes, d_sink, stream, qualities)
+        return PolishStream(self, capacity_bytes, d_sink, stream, qualities, edits, capacity_events, d_events)
 
 
 class PolishStream:
@@ -359,20 +364,41 @@ class PolishStream:
         per_group = s.group_bytes()      # bytes of each group, in run order
 
     `qualities=True` (pb_polish_stream_begin_qual): the sink holds 2-byte polish.QUAL_RECORD records (base, FASTQ quality
-    byte) in place of bytes, `d_sink` is 2 * `capacity_bytes` bytes, and every count of the session is in records."""
+    byte) in place of bytes, `d_sink` is 2 * `capacity_bytes` bytes, and every count of the session is in records.
 
-    def __init__(self, caller: PolishCaller, capacity_bytes: int, d_sink: int, stream: int = 0, qualities: bool = False):
+    `edits=True` (pb_polish_stream_edits): the session also writes the edit events of every group (polish_edits.EDIT_EVENT:
+    the winning columns that delete, substitute or insert, and one coverage record per image) to the device buffer `d_events`
+    (`capacity_events` events); `group_events()` gives the events of each group.  Groups are staged with their reference
+    (a FetchedReads), which the session holds until the group has been encoded."""
+
+    def __init__(self, caller: PolishCaller, capacity_bytes: int, d_sink: int, stream: int = 0, qualities: bool = False,
+                 edits: bool = False, capacity_events: int = 0, d_events: int = 0):
+        from collections import deque
         self.c, self.L = caller, caller.L
         self.capacity = int(capacity_bytes)
+        self.capacity_events = int(capacity_events)
+        self.edits = bool(edits)
         self.groups = 0
+        self._held = deque(maxlen=3)
         begin = self.L.pb_polish_stream_begin_qual if qualities else self.L.pb_polish_stream_begin
         _lib.check(begin(caller.enc.h, caller.net.h, self.capacity, C.c_void_p(d_sink or None), C.c_void_p(stream)),
                    "pb_polish_stream_begin_qual" if qualities else "pb_polish_stream_begin")
+        if self.edits:
+            _lib.check(self.L.pb_polish_stream_edits(caller.enc.h, self.capacity_events, C.c_void_p(d_events or None)),
+                       "pb_polish_stream_edits")
 
     def stage_device(self, dreads, g0: int, g1: int, region_id0: int = 0):
         """`dreads`: DeviceReads / FetchedReads whose region table the group indices [g0, g1) refer to."""
-        _lib.check(self.L.pb_polish_stream_stage_device(self.c.enc.h, C.byref(dreads.struct), dreads.h_regions, g0, g1, region_id0),
-                   "pb_polish_stream_stage_device")
+        if not self.edits:
+            _lib.check(self.L.pb_polish_stream_stage_device(self.c.enc.h, C.byref(dreads.struct), dreads.h_regions, g0, g1, region_id0),
+                       "pb_polish_stream_stage_device")
+            return
+        # the group is encoded by the run after this stage, and the run after that synchronises with the encoder: the
+        # reference (dreads' device tensors) must live until then
+        self._held.append(dreads)
+        _lib.check(self.L.pb_polish_stream_stage_device_draft(self.c.enc.h, C.byref(dreads.struct), dreads.h_regions, g0, g1,
+                                                              region_id0, C.c_void_p(dreads.d_ref)),
+                   "pb_polish_stream_stage_device_draft")
 
     def run(self, flush: bool = False) -> int:
         """Returns the encoded columns of the session so far: an upper bound of its consensus bytes."""
@@ -387,6 +413,12 @@ class PolishStream:
     def end(self) -> int:
         n = C.c_int64(0)
         rc = self.L.pb_polish_stream_end(self.c.enc.h, self.c.net.h, C.byref(n))
+        self._held.clear()
+        if rc == PB_ERR_CAPACITY and self.edits and n.value <= self.capacity:
+            need = self.event_total()
+            ex = _lib.PepperB200Error("edit event capacity %d too small (need %d events)" % (self.capacity_events, need), rc)
+            ex.need, ex.need_events = int(n.value), need
+            raise ex
         if rc == PB_ERR_CAPACITY:
             ex = _lib.PepperB200Error("consensus sink capacity %d too small (need %d bytes)" % (self.capacity, n.value), rc)
             ex.need = int(n.value)
@@ -397,6 +429,17 @@ class PolishStream:
     def group_bytes(self) -> np.ndarray:
         out = np.zeros(self.groups, np.int64)
         _lib.check(self.L.pb_polish_stream_group_bytes(self.c.enc.h, out.ctypes.data, self.groups), "pb_polish_stream_group_bytes")
+        return out
+
+    def event_total(self) -> int:
+        """Edit events the session needed (an edits session, after end())."""
+        n = C.c_int64(0)
+        _lib.check(self.L.pb_polish_stream_event_total(self.c.enc.h, C.byref(n)), "pb_polish_stream_event_total")
+        return int(n.value)
+
+    def group_events(self) -> np.ndarray:
+        out = np.zeros(self.groups, np.int64)
+        _lib.check(self.L.pb_polish_stream_group_events(self.c.enc.h, out.ctypes.data, self.groups), "pb_polish_stream_group_events")
         return out
 
     def stats(self) -> dict:

@@ -11,8 +11,12 @@ assembly against the single-GPU `polish_contig` of sampled contigs (`verified`).
 per-base qualities, the two modes alternating on one driver, and the line gains `fastq`: the wall time of every run, the
 polished bases/s of each mode (total bases over total wall), and whether the FASTQ sequences equal the FASTA sequences.
 
+`--vcf`: likewise with and without the edits VCF (edit events through the session and the all-gather, then the device record
+pass, compression and index of DistributedPolisher.write_edits, inside the timed run); the line gains `vcf`: the wall times,
+the polished bases/s of each mode, the records written, and whether the FASTA of the edits runs equals the plain FASTA.
+
     python scripts/bench_polish_assembly.py [--contigs 20] [--mb 5] [--coverage 40] [--group-regions 32] [--check 3]
-                                            [--fastq [--reps 3]]"""
+                                            [--fastq] [--vcf] [--reps 3]"""
 import argparse
 import json
 import os
@@ -62,7 +66,8 @@ def main():
     ap.add_argument("--check", type=int, default=3, help="contigs compared with polish_contig on rank 0")
     ap.add_argument("--seed", type=int, default=1)
     ap.add_argument("--fastq", action="store_true", help="also time the assembly with per-base qualities, alternating with FASTA")
-    ap.add_argument("--reps", type=int, default=3, help="--fastq: runs of each mode")
+    ap.add_argument("--vcf", action="store_true", help="also time the assembly with the edits VCF, alternating with FASTA")
+    ap.add_argument("--reps", type=int, default=3, help="--fastq / --vcf: runs of each mode")
     args = ap.parse_args()
 
     import torch
@@ -87,22 +92,28 @@ def main():
         cap = int(2.5 * draft / world) + (4 << 20)            # this rank's consensus slice (bytes)
         # warm-up on one contig: library buffers, first kernel launches, NCCL communicator
         wsrc = PolishFileSource(bam, fa, contigs=names[:1], device=local)
-        dp = DistributedPolisher(state, local, cap, args.schedule, args.group_regions)
-        for q in ([False, True] if args.fastq else [False]):
-            dp.qualities = q
+        # events: at most one per image column plus one per image; the seeded random weights edit most draft bases
+        dp = DistributedPolisher(state, local, cap, args.schedule, args.group_regions, capacity_events=cap)
+        vcf_path = os.path.join(tmp, "edits.vcf.gz")
+        for q, e in [(False, False)] + ([(True, False)] if args.fastq else []) + ([(False, True)] if args.vcf else []):
+            dp.qualities, dp.edits = q, e
             dp.run(wsrc)
-        dp.qualities = False
+            if e and rank == 0:
+                dp.write_edits(wsrc, vcf_path)
+        dp.qualities = dp.edits = False
         wsrc.close()
         src = PolishFileSource(bam, fa, device=local)
 
-        def timed(qualities: bool):
-            dp.qualities = qualities
+        def timed(qualities: bool, edits: bool = False):
+            dp.qualities, dp.edits = qualities, edits
             if world > 1:
                 dist.barrier()
             torch.cuda.synchronize()
             t = time.perf_counter()
             n = dp.run(src)
             out = dp.assemble(src)
+            if edits and rank == 0:
+                dp.write_edits(src, vcf_path)
             return n, out, time.perf_counter() - t
         n, seqs, wall = timed(False)
         mine = dict(dp.phase_ms, consensus_bytes=n, images=dp.stats.get("images", 0))
@@ -119,6 +130,23 @@ def main():
             fastq = dict(reps=args.reps, wall_s={k: [round(w, 3) for w in v] for k, v in walls.items()},
                          polished_bases_per_s={k: round(bases * len(v) / sum(v), 1) for k, v in walls.items()},
                          fastq_sequences_equal_fasta=bool(same))
+        vcf = None
+        if args.vcf:
+            import gzip
+            walls = {"fasta": [], "vcf": []}
+            same = True
+            for rep_ in range(args.reps):
+                for e in ((True, False) if rep_ % 2 == 0 else (False, True)):
+                    _, out, w = timed(False, e)
+                    walls["vcf" if e else "fasta"].append(w)
+                    same = same and out == seqs
+            bases = sum(len(s) for s in seqs.values())
+            records = None
+            if rank == 0:
+                records = sum(1 for ln in gzip.decompress(open(vcf_path, "rb").read()).split(b"\n") if ln and not ln.startswith(b"#"))
+            vcf = dict(reps=args.reps, wall_s={k: [round(w, 3) for w in v] for k, v in walls.items()},
+                       polished_bases_per_s={k: round(bases * len(v) / sum(v), 1) for k, v in walls.items()},
+                       records=records, vcf_fasta_equals_fasta=bool(same))
         per_rank = [None] * world
         if world > 1:
             dist.all_gather_object(per_rank, mine)
@@ -142,7 +170,7 @@ def main():
                 wall_s=round(wall, 3), polished_bases_per_s=round(polished / wall, 1), draft_bases_per_s=round(draft / wall, 1),
                 per_rank=[{k: (round(v, 2) if isinstance(v, float) else v) for k, v in r.items()} for r in per_rank],
                 card=torch.cuda.get_device_name(local), power_limit_w=power_limit_w(local), synth_s=round(gen_s, 1),
-                verified=verified, **({"fastq": fastq} if args.fastq else {}))), flush=True)
+                verified=verified, **({"fastq": fastq} if args.fastq else {}), **({"vcf": vcf} if args.vcf else {}))), flush=True)
     finally:
         shutil.rmtree(tmp, ignore_errors=True)
         if world > 1:
