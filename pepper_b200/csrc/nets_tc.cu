@@ -250,7 +250,7 @@ static int variant_lstm_layer_tc(pb_variant_net *N, int layer, int64_t B, bool l
         }
         L.y_hi = y_hi; L.y_lo = y_lo; L.y_mt_stride = y_mt_stride;
         if (y_f32) { L.y_f32 = y_f32; L.ldy = (int64_t) VT * 512; }
-        L.M = (int) B; L.n_mt = (int) Mt; L.T = VT; L.c_ld = Bp;
+        L.M = (int) B; L.n_mt = (int) Mt; L.T = VT;
         L.lo_x = lo_x; L.lo_h = lo_h;
         if (q8) {
             if (layer != 0 || lo_h) { set_error("int8 slice output: encoder layer with a hi-only h-part"); return PB_ERR_STATE; }
@@ -274,7 +274,7 @@ static int variant_lstm_layer_tc(pb_variant_net *N, int layer, int64_t B, bool l
     if (q8) { set_error("int8 slice output needs the persistent encoder kernel"); return PB_ERR_STATE; }
     for (int t = 0; t < VT; t++) {
         Args A;
-        A.M = (int) B; A.N = 4 * VH; A.c_ld = Bp;
+        A.M = (int) B; A.N = 4 * VH;
         for (int d = 0; d < 2; d++) {
             const int tt = d == 0 ? t : VT - 1 - t;
             const int tp = d == 0 ? tt - 1 : tt + 1;
@@ -318,7 +318,11 @@ static int variant_dec_q8(pb_variant_net *N, int64_t B, bool persist, float *y_f
         L.c[d] = T.c.as<float>() + (int64_t) d * VH * Bp;
     }
     if (y_f32) { L.y_f32 = y_f32; L.ldy = (int64_t) VT * 512; }
-    L.M = (int) B; L.n_mt = (int) Mt; L.T = VT; L.c_ld = Bp;
+    L.M = (int) B; L.n_mt = (int) Mt; L.T = VT;
+#ifdef PB_LSTM_TRACE
+    PB_TRY(lstm_trace_buffer(1, &L.trace));
+    PB_CUDA(cudaMemsetAsync(L.trace, 0, sizeof(uint64_t) * tc::lstm_trace_words(VT), st));
+#endif
     static bool attr_set = false;
     if (!attr_set) {
         PB_CUDA(cudaFuncSetAttribute(tc::k_lstm_layer_q8, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::QSMEM_BYTES));
@@ -444,7 +448,7 @@ int variant_forward_tc(pb_variant_net *N, const int8_t *d_images, int64_t B, flo
             continue;
         }
         Args A;
-        A.M = (int) B; A.N = 512; A.c_ld = 0;
+        A.M = (int) B; A.N = 512;
         Dir D = empty_dir();
         if (i == 0) {
             D.seg[0].hi = T.ydec_hi.as<bf16>(); D.seg[0].lo = ((T.lo_mask >> 3) & 1) ? T.ydec_lo.as<bf16>() : nullptr;
@@ -693,7 +697,7 @@ extern "C" int pb_test_tc_gemm_ex(int M, int N, int epi, int K0, const float *h_
     TcLin W;
     int rc = tc_upload_lin(W, h_W, h_bias, N, K0 + K1);
     Args A;
-    A.M = M; A.N = N; A.c_ld = 0;
+    A.M = M; A.N = N;
     Dir D = empty_dir();
     D.seg[0].hi = a0hi.as<bf16>(); D.seg[0].lo = lo0 ? a0lo.as<bf16>() : nullptr; D.seg[0].mt_stride = (int64_t) (K0 / 32) * TILE_ELEMS; D.seg[0].nkt = K0 / 32;
     if (K1) { D.seg[1].hi = a1hi.as<bf16>(); D.seg[1].lo = lo1 ? a1lo.as<bf16>() : nullptr; D.seg[1].mt_stride = (int64_t) (K1 / 32) * TILE_ELEMS; D.seg[1].nkt = K1 / 32; }
@@ -730,6 +734,17 @@ extern "C" int pb_test_tc_gemm_ex(int M, int N, int epi, int K0, const float *h_
 // C[M][N] = A[M][K] W[N][K]^T + bias through the wgmma kernel (EPI_BIAS, fp32 output).  N % 256 == 0, K % 32 == 0.
 extern "C" int pb_test_tc_gemm(int M, int N, int K, const float *h_A, const float *h_W, const float *h_bias, float *h_out) {
     return pb_test_tc_gemm_ex(M, N, tc::EPI_BIAS, K, h_A, 1, 0, nullptr, 0, h_W, h_bias, 0, 0, h_out, nullptr, nullptr);
+}
+
+// The cell state the last variant LSTM layer left in T.c (tc::c_index per direction) as c_final [2][256][M].
+static int read_c_final(TcVariant &T, int M, float *h_c_final) {
+    const int64_t per_dir = ceil_div(M, 128) * 128 * VH;
+    std::vector<float> c((size_t) (2 * per_dir));
+    PB_CUDA(cudaMemcpy(c.data(), T.c.p, sizeof(float) * c.size(), cudaMemcpyDeviceToHost));
+    for (int d = 0; d < 2; d++)
+        for (int u = 0; u < VH; u++)
+            for (int r = 0; r < M; r++) h_c_final[((size_t) d * VH + u) * M + r] = c[d * per_dir + tc::c_index(u, r)];
+    return PB_OK;
 }
 
 // One LSTM layer of the variant network (variant_lstm_layer_tc, the forward pass's own launch code) with the network's packed
@@ -774,10 +789,7 @@ extern "C" int pb_test_variant_lstm_layer(pb_variant_net_t *net, int layer, int 
         PB_CUDA(cudaMemcpy(h_y_hi, (layer == 0 ? T.yenc_hi : T.ydec_hi).p, (size_t) seq * 2, cudaMemcpyDeviceToHost));
         PB_CUDA(cudaMemcpy(h_y_lo, (layer == 0 ? T.yenc_lo : T.ydec_lo).p, (size_t) seq * 2, cudaMemcpyDeviceToHost));
     }
-    if (h_c_final)
-        for (int d = 0; d < 2; d++)
-            PB_CUDA(cudaMemcpy2D(h_c_final + (size_t) d * VH * M, sizeof(float) * M, T.c.as<float>() + (int64_t) d * VH * Bp,
-                                 sizeof(float) * Bp, sizeof(float) * M, VH, cudaMemcpyDeviceToHost));
+    if (h_c_final) PB_TRY(read_c_final(T, M, h_c_final));
     return PB_OK;
 }
 
@@ -787,7 +799,7 @@ extern "C" int pb_test_variant_lstm_q8(pb_variant_net_t *net, int M, const float
     if (!net || M <= 0 || !h_x) { set_error("pb_test_variant_lstm_q8: bad argument"); return PB_ERR_ARG; }
     PB_CUDA(cudaSetDevice(net->device));
     TcVariant &T = net->tc;
-    const int64_t Mt = ceil_div(M, 128), Bp = Mt * 128, qbytes = Mt * q_mt_bytes();
+    const int64_t Mt = ceil_div(M, 128), qbytes = Mt * q_mt_bytes();
     PB_TRY(variant_reserve_tc(T, M, 2));
     if (poison) {
         DevBuf *bufs[] = {&T.yenc_lo, &T.ydec_q, &T.c};
@@ -812,10 +824,7 @@ extern "C" int pb_test_variant_lstm_q8(pb_variant_net_t *net, int M, const float
     PB_CUDA(cudaDeviceSynchronize());
     if (h_y_f32) PB_CUDA(cudaMemcpy(h_y_f32, S.b[0].p, sizeof(float) * (size_t) M * VT * 512, cudaMemcpyDeviceToHost));
     if (h_q) PB_CUDA(cudaMemcpy(h_q, T.ydec_q.p, (size_t) (2 * qbytes), cudaMemcpyDeviceToHost));
-    if (h_c_final)
-        for (int d = 0; d < 2; d++)
-            PB_CUDA(cudaMemcpy2D(h_c_final + (size_t) d * VH * M, sizeof(float) * M, T.c.as<float>() + (int64_t) d * VH * Bp,
-                                 sizeof(float) * Bp, sizeof(float) * M, VH, cudaMemcpyDeviceToHost));
+    if (h_c_final) PB_TRY(read_c_final(T, M, h_c_final));
     return PB_OK;
 }
 

@@ -73,7 +73,7 @@ struct Dir {
     int w_nkt;                          // k-tiles per n-tile of the packed weight (>= k-tiles of this launch)
     const float *bias;                  // [N]
     float inv_scale;                    // 1 / s of the packed weight (TcRnn / TcLin::scale): acc * inv_scale + bias, exact
-    float *c;                           // LSTM cell state [H][c_ld]
+    float *c;                           // LSTM cell state of 256 units, lane-owned (c_index)
     op_t *y_hi, *y_lo;                  // output operand tiles: tile (mt, y_kt0 + col/32)
     int64_t y_mt_stride;
     int y_kt0;
@@ -82,8 +82,19 @@ struct Dir {
 struct Args {
     Dir d[2];
     int M, N;                           // valid rows; N = columns of the packed weight (multiple of 256)
-    int64_t c_ld;
 };
+
+// Cell state of one direction of a 256-unit LSTM layer: 128 rows x 256 units = 32,768 floats per row tile, laid out so that
+// each consumer thread's cells are contiguous.  In every LSTM epilogue consumer thread ct = 32 warp + lane (0-255) owns row
+// r = 16 warp + lane / 4 + 8 (lane & 1) of its tile and units u with u & 1 = (lane >> 1) & 1; cell (u, r) sits at
+//   ((u / 8) * 256 + ct) * 4 + (u / 2) % 4
+// so a lane's four cells u / 8 = const go out as one 16 B access, and a warp's as 512 contiguous bytes.  A lane owns the
+// same cells at every step, and nothing outside the layer kernels reads them except the test hooks (through this function).
+__host__ __device__ __forceinline__ int64_t c_index(int unit, int64_t row) {
+    const int r = (int) (row & 127);
+    const int ct = (r >> 4) * 32 + (r & 7) * 4 + (unit & 1) * 2 + ((r >> 3) & 1);
+    return (row >> 7) * (BM * 256) + ((int64_t) (unit >> 3) * 256 + ct) * 4 + ((unit >> 1) & 3);
+}
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t) __cvta_generic_to_shared(p); }
 
@@ -391,12 +402,14 @@ __global__ void __launch_bounds__(PG_THREADS, 1) k_tc_gemm_p(Args G, int n_mt, i
         } else {
             const int r128 = rA + 8 * (q & 1), row = mt * BM + r128;
             const bool valid = row < G.M;
+            // unit nt * 64 + 2 i + q / 2 of this row sits at cl + (i / 4) * 1024 + i % 4 (c_index)
+            float *const cl = D.c + c_index(nt * (PBN / 4) + (q >> 1), row);
 #pragma unroll
             for (int i = 0; i < PBN / 8; i++) {
                 const int j = nt * (PBN / 4) + 2 * i + (q >> 1);
                 float gt[4];
                 gates4(acc, i, __ldg(reinterpret_cast<const float2 *>(D.bias + nt * PBN + 8 * i + 2 * q)), D.inv_scale, q, gt);
-                float *cp = D.c + (int64_t) j * G.c_ld + row;
+                float *cp = cl + (i >> 2) * 1024 + (i & 3);
                 const float cn = sigm(gt[1]) * (valid ? *cp : 0.f) + sigm(gt[0]) * tanh_fast(gt[2]);
                 if (valid) *cp = cn;
                 const float hn = sigm(gt[3]) * tanh_fast(cn);
@@ -426,13 +439,12 @@ struct LstmLayer {
     const op_t *w_hi[2], *w_lo[2];     // per direction: [4 n-tiles][x_nkt + 8][WTILE_ELEMS]
     const float *bias[2];
     float inv_scale[2];                // 1 / s of each direction's packed weight
-    float *c[2];                       // cell state per direction [256][c_ld], zero initialised
+    float *c[2];                       // cell state per direction (c_index), zero initialised
     op_t *y_hi, *y_lo;                 // output sequence operand [mt][T][16] tiles; (time tt, direction d) -> k-tiles tt * 16 + d * 8 ...
     int64_t y_mt_stride;
     float *y_f32;                      // optional fp32 copy [row][T][512]
     int64_t ldy;
     int M, n_mt, T;
-    int64_t c_ld;
     int lo_x, lo_h;                    // 1: the a_lo x w_hi product of the x-part / h-part is executed (0: two products)
     int8_t *q1, *q0;                   // k_lstm_layer<true>: h_t as int8 slices for the next layer instead of y_lo (QSeq layout)
     int64_t q_mt_stride;               // bytes
@@ -443,13 +455,14 @@ struct LstmLayer {
 
 #ifdef PB_LSTM_TRACE
 // Timing build only (-DPB_LSTM_TRACE; scripts/trace_lstm_layer.py): %clock64 stamps of CTAs 0, gridDim / 2 and
-// gridDim - 1.  Per sampled CTA, in 64-bit words (cw = consumer warp 0-7, nt = gate tile):
-//   [((cw * T + t) * 4 + nt) * 4 + k]  k: 0 tile start, 1 first bar_full passed, 2 wg_wait<0> returned, 3 epilogue end
-//   [128 T + (cw * T + t) * 2 + k]     k: 0 __threadfence returned, 1 bar_h arrived
-//   [144 T + t * 3 + k]                producer, t >= 1; k: 0 bar_h wait start, 1 wait end, 2 first h-part copy issued
-//   [147 T + k]                        k: 0 %globaltimer, 1 %clock64 at the start; 2, 3 the same when warp 0 ends
+// gridDim - 1 of k_lstm_layer and k_lstm_layer_q8.  Per sampled CTA, in 64-bit words (cw = consumer warp 0-7, nt = gate
+// tile: 0-3 in k_lstm_layer, 0-7 in k_lstm_layer_q8):
+//   [((cw * T + t) * 8 + nt) * 4 + k]  k: 0 tile start, 1 first bar_full passed, 2 wg_wait<0> returned, 3 epilogue end
+//   [256 T + (cw * T + t) * 2 + k]     k: 0 __threadfence returned, 1 bar_h arrived
+//   [272 T + t * 3 + k]                producer, t >= 1; k: 0 bar_h wait start, 1 wait end, 2 first h-part copy issued
+//   [275 T + k]                        k: 0 %globaltimer, 1 %clock64 at the start; 2, 3 the same when warp 0 ends
 constexpr int LSTM_TRACE_CTAS = 3;
-__host__ __device__ constexpr int64_t lstm_trace_cta_words(int T) { return 147 * (int64_t) T + 4; }
+__host__ __device__ constexpr int64_t lstm_trace_cta_words(int T) { return 275 * (int64_t) T + 4; }
 __host__ __device__ constexpr int64_t lstm_trace_words(int T) { return LSTM_TRACE_CTAS * lstm_trace_cta_words(T); }
 __device__ __forceinline__ uint64_t trace_clock() {
     uint64_t c;
@@ -491,7 +504,7 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
 #ifdef PB_LSTM_TRACE
     const int ts = blockIdx.x == 0 ? 0 : blockIdx.x == gridDim.x / 2 ? 1 : blockIdx.x == gridDim.x - 1 ? 2 : -1;
     uint64_t *const tr = G.trace && ts >= 0 ? G.trace + ts * lstm_trace_cta_words(G.T) : nullptr;
-    if (tr && threadIdx.x == 0) { tr[147 * G.T] = trace_gtime(); tr[147 * G.T + 1] = trace_clock(); }
+    if (tr && threadIdx.x == 0) { tr[275 * G.T] = trace_gtime(); tr[275 * G.T + 1] = trace_clock(); }
 #endif
     __syncthreads();
 
@@ -512,17 +525,17 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
                             const int kk = kt - G.x_nkt;
                             if (kk == 0 && nt == 0) {
                                 // every consumer warp has written its part of h_{t-1}: make it visible to the bulk-copy engine
-                                LSTM_STAMP(144 * G.T + t * 3);
+                                LSTM_STAMP(272 * G.T + t * 3);
                                 mbar_wait(bar_h, (uint32_t) (t - 1) & 1u);
                                 asm volatile("fence.proxy.async;" ::: "memory");
-                                LSTM_STAMP(144 * G.T + t * 3 + 1);
+                                LSTM_STAMP(272 * G.T + t * 3 + 1);
                             }
                             const int64_t off = (int64_t) mt * G.y_mt_stride + ((int64_t) tp * 16 + dir * 8 + kk) * TILE_ELEMS;
                             a_hi = G.y_hi + off; a_lo = G.lo_h ? G.y_lo + off : nullptr;
                         }
                         const int64_t woff = ((int64_t) nt * w_nkt + kt) * WTILE_ELEMS;
                         load_stage(smem_base, bar_full, bar_empty, g, a_hi, a_lo, G.w_hi[dir] + woff, G.w_lo[dir] + woff);
-                        if (t > 0 && nt == 0 && kt == G.x_nkt) LSTM_STAMP(144 * G.T + t * 3 + 2);
+                        if (t > 0 && nt == 0 && kt == G.x_nkt) LSTM_STAMP(272 * G.T + t * 3 + 2);
                     }
                 }
             }
@@ -536,7 +549,7 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
     const bool valid = row < G.M;
     const bool lo_x = G.x_lo != nullptr && G.lo_x != 0, lo_h = G.lo_h != 0;
     const float inv_s = G.inv_scale[dir];
-    const int c2 = 2 * (int) G.c_ld;                                  // cell state of unit j + 2 lies c2 floats after unit j
+    float4 *const cl = reinterpret_cast<float4 *>(G.c[dir] + c_index(q >> 1, row));   // this lane's first four cells
     uint32_t g = 0;
     float acc[128];
     for (int t = 0; t < G.T; t++) {
@@ -545,24 +558,23 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
         const int64_t y0 = (int64_t) mt * G.y_mt_stride + (int64_t) (tt * 16 + dir * 8) * TILE_ELEMS + r128 * 8;
         for (int nt = 0; nt < 4; nt++) {
 #ifdef PB_LSTM_TRACE
-            const int tc0 = ((warp * G.T + t) * 4 + nt) * 4;
+            const int tc0 = ((warp * G.T + t) * 8 + nt) * 4;
 #endif
             LSTM_STAMP(tc0);
-            // cell states of units nt * 64 + 2 i + q / 2, in flight during the k-loop
-            float *cp = G.c[dir] + (int64_t) (nt * (PBN / 4) + (q >> 1)) * G.c_ld + row;
+            // cell states of units nt * 64 + 2 i + q / 2 (cells 4 k .. 4 k + 3 in one float4), in flight during the k-loop
+            float4 *cp = cl + nt * (PBN / 32) * 256;
             float c_prev[PBN / 8];
 #pragma unroll
-            for (int i = 0; i < PBN / 8; i++) c_prev[i] = valid ? __ldcg(cp + i * c2) : 0.f;
+            for (int k = 0; k < PBN / 32; k++) {
+                const float4 v = valid ? __ldcg(cp + k * 256) : make_float4(0.f, 0.f, 0.f, 0.f);
+                c_prev[4 * k] = v.x; c_prev[4 * k + 1] = v.y; c_prev[4 * k + 2] = v.z; c_prev[4 * k + 3] = v.w;
+            }
 #ifdef PB_LSTM_TRACE
             mbar_wait(bar_full + 8 * (g % PSTAGES), (g / PSTAGES) & 1u);     // mma_tile's first wait then passes at once
             LSTM_STAMP(tc0 + 1);
 #endif
             mma_tile(acc, smem_base, bar_full, bar_empty, g, nkt, G.x_nkt, lo_x, lo_h, wg, lane);
             LSTM_STAMP(tc0 + 2);
-            // the stores recompute their addresses (IMAD per cell) instead of keeping the 32 load pointers alive across
-            // the k-loop
-            int c2s;
-            asm volatile("mov.b32 %0, %1;" : "=r"(c2s) : "r"(c2));
             const float *sb = sbias + nt * PBN + 2 * q;
             // units nt * 64 .. + 63 are operand k-tiles 2 nt, 2 nt + 1 of this step.  Lanes q and q ^ 2 hold units 2 i and
             // 2 i + 1 of the same row: the even-unit lane writes the hi words of the pair, the odd-unit lane the lo words.
@@ -586,7 +598,7 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
                     gates4(acc, i, *reinterpret_cast<const float2 *>(sb + 8 * i), inv_s, q, gt);
                     const float cn = sigm(gt[1]) * c_prev[i] + sigm(gt[0]) * tanh_fast(gt[2]);
                     const float hn = sigm(gt[3]) * tanh_fast(cn);
-                    if (valid) cp[i * c2s] = cn;
+                    c_prev[i] = cn;
                     const float hp = __shfl_xor_sync(0xffffffffu, hn, 2);
                     const float h0 = odd_u ? hp : hn, h1 = odd_u ? hn : hp;          // units 2 i, 2 i + 1
                     if constexpr (Q8) {
@@ -607,18 +619,23 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
                     // element (unit nt * 64 + 4 m, row r128) of the step's operand tiles, relative to the lane's base
                     if (valid) __stwb(reinterpret_cast<uint2 *>(yw + (m >> 3) * TILE_ELEMS + ((m >> 1) & 3) * 1024 + 4 * (m & 1)), make_uint2(w[0], w[1]));
                 }
+                // cells 2 m - 2 .. 2 m + 1 are done: one 16 B store
+                if ((m & 1) && valid) {
+                    const int k = m >> 1;
+                    cp[k * 256] = make_float4(c_prev[4 * k], c_prev[4 * k + 1], c_prev[4 * k + 2], c_prev[4 * k + 3]);
+                }
             }
             LSTM_STAMP(tc0 + 3);
         }
         // h_t of this warp's rows is complete (all four gate tiles): publish it to the producer thread
         __threadfence();
-        LSTM_STAMP(128 * G.T + (warp * G.T + t) * 2);
+        LSTM_STAMP(256 * G.T + (warp * G.T + t) * 2);
         __syncwarp();
         if (lane == 0) mbar_arrive(bar_h);
-        LSTM_STAMP(128 * G.T + (warp * G.T + t) * 2 + 1);
+        LSTM_STAMP(256 * G.T + (warp * G.T + t) * 2 + 1);
     }
 #ifdef PB_LSTM_TRACE
-    if (tr && threadIdx.x == 0) { tr[147 * G.T + 2] = trace_gtime(); tr[147 * G.T + 3] = trace_clock(); }
+    if (tr && threadIdx.x == 0) { tr[275 * G.T + 2] = trace_gtime(); tr[275 * G.T + 3] = trace_clock(); }
 #endif
 }
 
@@ -634,13 +651,15 @@ struct LstmLayerQ {
     const int8_t *w1[2], *w0[2];       // per direction: [8 n-tiles][12 k-tiles][QTILE_BYTES]
     const float *bias[2];
     const float *col_scale[2];         // [1024] 256 / (32512 sw_n)
-    float *c[2];                       // cell state per direction [256][c_ld]
+    float *c[2];                       // cell state per direction (c_index)
     int8_t *q1, *q0;                   // output sequence slices (QSeq); direction d -> k-tiles 4 d .. 4 d + 3
     int64_t q_mt_stride;               // bytes, the same for x and q
     float *y_f32;                      // optional fp32 copy [row][T][512]
     int64_t ldy;
     int M, n_mt, T, t0, t1;
-    int64_t c_ld;
+#ifdef PB_LSTM_TRACE
+    uint64_t *trace;                   // lstm_trace_words(T) stamps per launch, nullptr: none
+#endif
 };
 
 __device__ __forceinline__ void load_stage_q(uint32_t smem_base, uint32_t bar_full, uint32_t bar_empty, uint32_t g, const int8_t *a1,
@@ -672,6 +691,11 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer_q8(LstmLayerQ G)
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     for (int i = threadIdx.x; i < 1024; i += LSTM_THREADS) { sbias[i] = G.bias[dir][i]; sscale[i] = G.col_scale[dir][i]; }
+#ifdef PB_LSTM_TRACE
+    const int ts = blockIdx.x == 0 ? 0 : blockIdx.x == gridDim.x / 2 ? 1 : blockIdx.x == gridDim.x - 1 ? 2 : -1;
+    uint64_t *const tr = G.trace && ts >= 0 ? G.trace + ts * lstm_trace_cta_words(G.T) : nullptr;
+    if (tr && threadIdx.x == 0) { tr[275 * G.T] = trace_gtime(); tr[275 * G.T + 1] = trace_clock(); }
+#endif
     __syncthreads();
 
     if (warp >= CONS_WARPS) {
@@ -690,14 +714,17 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer_q8(LstmLayerQ G)
                         } else {
                             if (kt == X_NKT && nt == 0 && t > G.t0) {
                                 // every consumer warp has written its part of h_{t-1}: make it visible to the bulk-copy engine
+                                LSTM_STAMP(272 * G.T + t * 3);
                                 mbar_wait(bar_h, (uint32_t) (t - G.t0 - 1) & 1u);
                                 asm volatile("fence.proxy.async;" ::: "memory");
+                                LSTM_STAMP(272 * G.T + t * 3 + 1);
                             }
                             const int64_t off = (int64_t) mt * G.q_mt_stride + ((int64_t) tp * 8 + dir * 4 + kt - X_NKT) * QTILE_BYTES;
                             a1 = G.q1 + off; a0 = G.q0 + off;
                         }
                         const int64_t woff = ((int64_t) nt * W_NKT + kt) * QTILE_BYTES;
                         load_stage_q(smem_base, bar_full, bar_empty, g, a1, a0, G.w1[dir] + woff, G.w0[dir] + woff);
+                        if (t > G.t0 && nt == 0 && kt == X_NKT) LSTM_STAMP(272 * G.T + t * 3 + 2);
                     }
                 }
             }
@@ -710,22 +737,31 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer_q8(LstmLayerQ G)
     const int row = mt * BM + r128;
     const bool valid = row < G.M;
     const bool odd_u = q >> 1;
-    const int c2 = 2 * (int) G.c_ld;
+    float4 *const cl = reinterpret_cast<float4 *>(G.c[dir] + c_index(q >> 1, row));   // this lane's first four cells
     uint32_t g = 0;
     int hh[64], mix[64];
     for (int t = G.t0; t < G.t1; t++) {
         const int tt = dir ? G.T - 1 - t : t;
         const int nkt = X_NKT + (t > 0 ? W_NKT - X_NKT : 0);
         for (int nt = 0; nt < N_TILES; nt++) {
-            float *cp = G.c[dir] + (int64_t) (nt * (QN / 4) + (q >> 1)) * G.c_ld + row;
+#ifdef PB_LSTM_TRACE
+            const int tc0 = ((warp * G.T + t) * 8 + nt) * 4;
+#endif
+            LSTM_STAMP(tc0);
+            // cell states of units nt * 32 + 2 i + q / 2 (cells 4 k .. 4 k + 3 in one float4), in flight during the k-loop
+            float4 *cp = cl + nt * (QN / 32) * 256;
             float c_prev[QN / 8];
 #pragma unroll
-            for (int i = 0; i < QN / 8; i++) c_prev[i] = valid ? __ldcg(cp + i * c2) : 0.f;
+            for (int k = 0; k < QN / 32; k++) {
+                const float4 v = valid ? __ldcg(cp + k * 256) : make_float4(0.f, 0.f, 0.f, 0.f);
+                c_prev[4 * k] = v.x; c_prev[4 * k + 1] = v.y; c_prev[4 * k + 2] = v.z; c_prev[4 * k + 3] = v.w;
+            }
 #pragma unroll
             for (int i = 0; i < 64; i++) { hh[i] = 0; mix[i] = 0; }
             for (int kt = 0; kt < nkt; kt++, g++) {
                 const uint32_t s = g % QSTAGES, ph = (g / QSTAGES) & 1u;
                 mbar_wait(bar_full + 8 * s, ph);
+                if (kt == 0) LSTM_STAMP(tc0 + 1);
                 const uint32_t st = smem_base + s * QSTAGE_BYTES, a = st + (uint32_t) wg * 1024, b = st + 2 * QTILE_BYTES;
                 wg_fence();
 #pragma unroll
@@ -744,11 +780,10 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer_q8(LstmLayerQ G)
                 }
             }
             wg_wait<0>();
+            LSTM_STAMP(tc0 + 2);
             __syncwarp();
             if (lane == 0) mbar_arrive(bar_empty + 8 * ((g - 1) % QSTAGES));
 
-            int c2s;
-            asm volatile("mov.b32 %0, %1;" : "=r"(c2s) : "r"(c2));
             const float *sb = sbias + nt * QN + 2 * q, *ss = sscale + nt * QN + 2 * q;
             // units nt * 32 .. + 31: slice k-tile 4 dir + nt / 2 (chunks 2 (nt & 1), + 1).  The even-unit lane writes slice 1
             // of a unit pair, the odd-unit lane slice 0.
@@ -773,7 +808,7 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer_q8(LstmLayerQ G)
                     const float gg = (q & 1) ? v[2] : r0, go = (q & 1) ? v[3] : r1;
                     const float cn = sigm(gf) * c_prev[i] + sigm(gi) * tanh_fast(gg);
                     const float hn = sigm(go) * tanh_fast(cn);
-                    if (valid) cp[i * c2s] = cn;
+                    c_prev[i] = cn;
                     const float hp = __shfl_xor_sync(0xffffffffu, hn, 2);
                     const float h0 = odd_u ? hp : hn, h1 = odd_u ? hn : hp;          // units 2 i, 2 i + 1
                     uq[2 * e] = qbias(h0); uq[2 * e + 1] = qbias(h1);
@@ -781,13 +816,24 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer_q8(LstmLayerQ G)
                 }
                 // units nt * 32 + 4 m .. + 3 of row r128
                 if (valid) __stwb(reinterpret_cast<uint32_t *>(qw + (m >> 2) * 2048 + 4 * (m & 3)), qword(uq[0], uq[1], uq[2], uq[3], odd_u));
+                // cells 2 m - 2 .. 2 m + 1 are done: one 16 B store
+                if ((m & 1) && valid) {
+                    const int k = m >> 1;
+                    cp[k * 256] = make_float4(c_prev[4 * k], c_prev[4 * k + 1], c_prev[4 * k + 2], c_prev[4 * k + 3]);
+                }
             }
+            LSTM_STAMP(tc0 + 3);
         }
         // h_t of this warp's rows is complete (all eight gate tiles): publish it to the producer thread
         __threadfence();
+        LSTM_STAMP(256 * G.T + (warp * G.T + t) * 2);
         __syncwarp();
         if (lane == 0) mbar_arrive(bar_h);
+        LSTM_STAMP(256 * G.T + (warp * G.T + t) * 2 + 1);
     }
+#ifdef PB_LSTM_TRACE
+    if (tr && threadIdx.x == 0) { tr[275 * G.T + 2] = trace_gtime(); tr[275 * G.T + 3] = trace_clock(); }
+#endif
 }
 
 // ---------------------------------------------------------------- persistent GEMM on int8 slices (linear_1, mode 2)

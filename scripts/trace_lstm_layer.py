@@ -1,11 +1,13 @@
-"""Where the time of k_lstm_layer goes: per-phase %clock64 stamps of a PB_LSTM_TRACE build (tc_gemm.cuh), for both
-variant LSTM layers of one VariantNet.predict chunk at each size.
+"""Where the time of the LSTM layer kernels goes: per-phase %clock64 stamps of a PB_LSTM_TRACE build (tc_gemm.cuh), for
+both variant LSTM layers of one VariantNet.predict chunk at each size (the encoder's k_lstm_layer and the decoder's
+k_lstm_layer_q8, or k_lstm_layer in mode 1).
 
     python scripts/trace_lstm_layer.py [--sizes 8448 1408] [--lib TRACED.so] [--build-dir DIR] [--out FILE]
 
 Without --lib the traced library is built with `make EXTRA=-DPB_LSTM_TRACE` into --build-dir (default: a new temporary
 directory), never into the tree.  CTAs 0, n/2 and n-1 are sampled; every phase is the median (and mean) over those CTAs,
-their 8 consumer warps, steps 1..32 and the 4 gate tiles (producer phases: over CTAs and steps).  Times are SM cycles; the
+their 8 consumer warps, steps 1..32 and the gate tiles, 4 in k_lstm_layer and 8 in k_lstm_layer_q8 (producer phases: over
+CTAs and steps).  Times are SM cycles; the
 kernel's own clock (cycles over %globaltimer) is printed beside the card name, power limit and nvidia-smi's SM clock.
 """
 import argparse
@@ -21,7 +23,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 T = 33                  # PB_VARIANT_WINDOW: steps per layer
 CTAS = 3                # LSTM_TRACE_CTAS
-CTA_WORDS = 147 * T + 4  # lstm_trace_cta_words(T)
+CTA_WORDS = 275 * T + 4  # lstm_trace_cta_words(T)
 
 
 def build_traced(build_dir: str) -> str:
@@ -52,21 +54,23 @@ def phases(words: np.ndarray) -> dict:
     mhz = []
     for s in range(CTAS):
         w = words[s * CTA_WORDS:(s + 1) * CTA_WORDS].astype(np.int64)
-        meta = w[147 * T:147 * T + 4]
+        meta = w[275 * T:275 * T + 4]
         if meta[1] == 0:
             continue
         if meta[2] > meta[0]:
             mhz.append((meta[3] - meta[1]) / (meta[2] - meta[0]) * 1e3)
-        tile = w[:128 * T].reshape(8, T, 4, 4)            # [warp][t][nt][start, first full, mma done, epilogue end]
-        step = w[128 * T:144 * T].reshape(8, T, 2)         # [warp][t][fence returned, bar_h arrived]
-        prod = w[144 * T:147 * T].reshape(T, 3)            # [t][bar_h wait start, wait end, first h copy issued]
+        tile = w[:256 * T].reshape(8, T, 8, 4)            # [warp][t][nt][start, first full, mma done, epilogue end]
+        if not tile[:, :, 4:].any():                       # k_lstm_layer: 4 gate tiles per step
+            tile = tile[:, :, :4]
+        step = w[256 * T:272 * T].reshape(8, T, 2)         # [warp][t][fence returned, bar_h arrived]
+        prod = w[272 * T:275 * T].reshape(T, 3)            # [t][bar_h wait start, wait end, first h copy issued]
         tl = tile[:, 1:]
         add("tile: start -> first bar_full", tl[..., 1] - tl[..., 0])
         add("tile: first bar_full -> wg_wait<0>", tl[..., 2] - tl[..., 1])
         add("tile: wg_wait<0> -> epilogue end", tl[..., 3] - tl[..., 2])
         add("tile: epilogue end -> next tile start", tl[:, :, 1:, 0] - tl[:, :, :-1, 3])
         add("tile period (start -> next start, same step)", tl[:, :, 1:, 0] - tl[:, :, :-1, 0])
-        add("step: last epilogue end -> __threadfence returned", step[:, 1:, 0] - tile[:, 1:, 3, 3])
+        add("step: last epilogue end -> __threadfence returned", step[:, 1:, 0] - tile[:, 1:, -1, 3])
         add("step: __threadfence -> bar_h arrived", step[:, 1:, 1] - step[:, 1:, 0])
         add("step: bar_h arrived -> next step's first tile start", tile[:, 2:, 0, 0] - step[:, 1:-1, 1])
         add("step period (tile 0 start -> next tile 0 start)", tile[:, 2:, 0, 0] - tile[:, 1:-1, 0, 0])
