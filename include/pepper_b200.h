@@ -542,6 +542,16 @@ int pb_variant_stream_stats(pb_variant_encoder_t *enc, float *ms5, int64_t *laun
 int pb_variant_stream_columns(pb_variant_encoder_t *enc, pb_candidate_columns_t *cols, const float **d_probs, const int8_t **d_images);
 int pb_variant_stream_fetch(pb_variant_encoder_t *enc, int64_t n, int8_t *h_images, int64_t *h_positions, uint8_t *h_depths,
                             uint8_t *h_freqs, char *h_keys, int32_t *h_region_of, float *h_probs, void *stream);
+/* gVCF track of a session: k_tile_count writes one uint32 (n_ref | n_alt << 16, each saturated at 65,535) per owned
+ * position of every region it encodes, regions in run order, each region's positions [cand_start, owned_end] back to back.
+ * Attach after _begin and before the first stage; after each stage give the staged group's owned ends (one per region,
+ * absolute and inclusive; cand_start - 1 for a region that owns nothing).  run() returns PB_ERR_CAPACITY, before it encodes
+ * the group, when the track could not hold it.  Without a track nothing changes. */
+int pb_variant_stream_track(pb_variant_encoder_t *enc, int64_t capacity_positions, uint32_t *d_track);
+int pb_variant_stream_owned(pb_variant_encoder_t *enc, const int64_t *h_owned_end, int64_t n);
+/* *n_positions: track positions written; *n_needed (optional): positions needed, above the capacity after a run() whose
+ * group did not fit the track (PB_ERR_CAPACITY from the track, as opposed to the candidate capacity) */
+int pb_variant_stream_track_used(pb_variant_encoder_t *enc, int64_t *n_positions, int64_t *n_needed);
 
 /* Fused make_images + call_consensus for the polish path (polish.py:14 steps
  * 1+2): encode, chunk into 1000-column images with 50 overlap
@@ -793,6 +803,49 @@ int pb_test_vcf_qual(const float *h_p, int64_t n, int32_t *h_qual);
  * d_sel / d_dst [n] are device arrays. */
 int pb_vcf_gather_lines_device(const char *d_text, const pb_vcf_line_t *d_lines, const int64_t *d_sel, const int64_t *d_dst,
                                int64_t n, uint8_t *d_out, void *stream);
+
+/* ------------------------------------------------------------------------
+ * gVCF reference blocks (DESIGN.md section 4, "gVCF").  Over a track of (n_ref, n_alt) pairs (pb_variant_stream_track)
+ * cut into segments (one per interval's owned window; a block never crosses a segment start) and half-open track ranges
+ * that are masked (written records' spans, positions before an earlier group's last record end): per position
+ * PL / GQ of the binomial reference-confidence model with log10 terms A = log10(1 - e), B = log10(e), H = log10(0.5),
+ * key = -1 at DP 0, else GQ / binsize; one block per maximal unmasked run of one key inside one segment.  Block lines:
+ *   CHROM POS . REF <*> . . END=<last> GT:GQ:MIN_DP:PL 0/0:<min GQ>:<min DP>:<PL of the first min-GQ position>
+ * (./.:0:0:0,0,0 for key -1), in track order; pb_vcf_line_t per block: pos, text_off, contig, ref_len = block length,
+ * cls = PB_GVCF_CLASS_BLOCK, text_len.  *n_text / *n_lines: the exact need (PB_ERR_CAPACITY when short, nothing written).
+ * ---------------------------------------------------------------------- */
+#define PB_GVCF_CLASS_BLOCK 3
+typedef struct {
+    int64_t toff;      /* track index of the segment's first position */
+    int64_t pos0;      /* its 0-based position */
+    int64_t len;       /* positions */
+    int64_t ref_off;   /* offset of pos0's reference base in d_ref */
+    int32_t contig;    /* contig id (index into the names) */
+    int32_t pad;
+} pb_gvcf_segment_t;
+typedef struct {
+    double a, b, h;    /* log10(1 - e), log10(e), log10(0.5) */
+    int32_t binsize;
+    int32_t pad;
+} pb_gvcf_params_t;
+/* h_segments [n_segments] and h_masks [n_masks][2] are host arrays; d_track, d_ref device arrays; h_names holds the
+ * contig names back to back, h_name_off [n_contigs + 1] */
+int pb_gvcf_blocks_device(const uint32_t *d_track, int64_t n_track, const pb_gvcf_segment_t *h_segments, int64_t n_segments,
+                          const int64_t *h_masks, int64_t n_masks, const char *d_ref, const char *h_names,
+                          const int64_t *h_name_off, int64_t n_contigs, const pb_gvcf_params_t *params, char *d_text,
+                          int64_t text_cap, pb_vcf_line_t *d_lines, int64_t lines_cap, int64_t *n_text, int64_t *n_lines,
+                          void *stream);
+/* the same over host arrays (h_ref: ref_bytes bytes) */
+int pb_gvcf_blocks_host(const uint32_t *h_track, int64_t n_track, const pb_gvcf_segment_t *h_segments, int64_t n_segments,
+                        const int64_t *h_masks, int64_t n_masks, const char *h_ref, int64_t ref_bytes, const char *h_names,
+                        const int64_t *h_name_off, int64_t n_contigs, const pb_gvcf_params_t *params, char *h_text,
+                        int64_t text_cap, pb_vcf_line_t *h_lines, int64_t lines_cap, int64_t *n_text, int64_t *n_lines,
+                        void *stream);
+/* gVCF record lines: line i of d_lines (a PEPPER_VARIANT_FULL line of d_text) is copied to d_out + d_out_off[i] with ",<*>"
+ * appended to ALT and ",." to each Number=A sample value (AP, AD, VAF): text_len + 10 bytes.  d_out_off [n] is a device
+ * array. */
+int pb_gvcf_records_device(const char *d_text, const pb_vcf_line_t *d_lines, int64_t n, const int64_t *d_out_off, char *d_out,
+                           void *stream);
 
 /* ------------------------------------------------------------------------
  * BGZF compression on the GPU (SAMv1 §4.1).  Member k is the payload bytes [member_off[k], member_off[k+1]) (at most

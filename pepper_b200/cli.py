@@ -2,6 +2,7 @@
 `pepper polish`:
 
     python -m pepper_b200 call_variant -b reads.bam -f ref.fa -m model.pkl -o out/ -s SAMPLE -t 16 --ont_r9_guppy5_sup
+    python -m pepper_b200 call_variant_gvcf ... (call_variant's flags) [--gvcf_gq_binsize 5]   # + PEPPER_VARIANT.g.vcf.gz
     python -m pepper_b200 polish -b reads.bam -f draft.fa -m model.pkl -o out/asm -t 16 [--fastq]
 
 Everything runs on the GPU (the device pipelines of frontend / dist).  With `-g`, one worker process per device of `-d_ids`
@@ -105,11 +106,16 @@ def build_parser() -> argparse.ArgumentParser:
     sub = parser.add_subparsers(dest="sub_command")
     add_call_variant_arguments(sub.add_parser("call_variant", help="BAM + FASTA -> the five PEPPER_VARIANT VCFs."))
     add_polish_arguments(sub.add_parser("polish", help="BAM + draft FASTA -> polished FASTA (and FASTQ)."))
+    g = add_call_variant_arguments(sub.add_parser("call_variant_gvcf", help="call_variant, and the gVCF PEPPER_VARIANT.g.vcf.gz."))
+    g.add_argument("--gvcf_gq_binsize", type=int, default=5,
+                   help="GQ band width of the gVCF's reference blocks: a block's positions share GQ // binsize. Default is 5.")
     return parser
 
 
+VARIANT_COMMANDS = ("call_variant", "call_variant_gvcf")
 NO_EFFECT = dict(call_variant=("batch_size", "num_workers", "callers_per_gpu", "quantized", "region_bed"),
                  polish=("batch_size", "num_workers"))
+NO_EFFECT["call_variant_gvcf"] = NO_EFFECT["call_variant"]
 
 
 def resolve(ns: argparse.Namespace) -> argparse.Namespace:
@@ -127,7 +133,7 @@ def no_effect_flags(parser: argparse.ArgumentParser, ns: argparse.Namespace) -> 
 
 
 # ----------------------------------------------------------------------------------------------------------- checks
-MODEL_KIND = dict(call_variant="variant", polish="polish")
+MODEL_KIND = dict(call_variant="variant", call_variant_gvcf="variant", polish="polish")
 
 
 def check_inputs(ns: argparse.Namespace) -> None:
@@ -156,6 +162,8 @@ def check_inputs(ns: argparse.Namespace) -> None:
         raise CliError("downsample_rate NEEDS TO BE IN (0, 1].")
     if getattr(ns, "region_size", 1) <= 0:
         raise CliError("region_size NEEDS TO BE >0.")
+    if getattr(ns, "gvcf_gq_binsize", 1) <= 0:
+        raise CliError("gvcf_gq_binsize NEEDS TO BE >0.")
 
 
 def load_model(path: str, kind: str) -> dict:
@@ -249,6 +257,7 @@ def run_call_variant(ns: argparse.Namespace, state: dict, device: int, distribut
     from .dist import DistributedGenomeCaller
     from .exclude import excluded_contigs
     from .frontend import VariantGenomeSource
+    from .gvcf import track_capacity
     from .pipeline import VariantCaller
     import torch.distributed as dist
     world, rank = (dist.get_world_size(), dist.get_rank()) if distributed else (1, 0)
@@ -277,8 +286,14 @@ def run_call_variant(ns: argparse.Namespace, state: dict, device: int, distribut
         opened.append(1)
         return src
 
+    gvcf = ns.sub_command == "call_variant_gvcf"
+
     def run(src, cap):
-        dgc = DistributedGenomeCaller(None, device, cap, "dynamic", distributed=distributed, caller=caller)
+        # the gVCF track grows with the candidate room: a restart doubles both
+        bases = sum(e - s + 1 for s, e in src.intervals)
+        track = track_capacity(bases, world) * (cap // variant_capacity(bases, world)) if gvcf else None
+        dgc = DistributedGenomeCaller(None, device, cap, "dynamic", distributed=distributed, caller=caller, gvcf=gvcf,
+                                      gvcf_binsize=getattr(ns, "gvcf_gq_binsize", 5), track_positions=track)
         try:
             return dgc.call_source(src, ns.output_dir, ns.sample_name, params, presets.candidate_options(vars(ns)),
                                    presets.vcf_options(vars(ns)))
@@ -287,7 +302,7 @@ def run_call_variant(ns: argparse.Namespace, state: dict, device: int, distribut
     caller = VariantCaller(state, device)
     try:
         return run_restarting(open_source, run, lambda src: variant_capacity(sum(e - s + 1 for s, e in src.intervals), world),
-                              world, "CANDIDATE")
+                              world, "CANDIDATE AND GVCF TRACK" if gvcf else "CANDIDATE")
     finally:
         caller.close()
 
@@ -357,9 +372,11 @@ TOTALS = ("TOTAL CANDIDATES FOUND", "TOTAL VARIANTS IN PEPPER", "TOTAL VARIANTS 
 
 def finish(ns: argparse.Namespace, result, t0: float) -> None:
     """Rank 0's output: the totals lines of call_variant; the polished files of polish."""
-    if ns.sub_command == "call_variant":
+    if ns.sub_command in VARIANT_COMMANDS:
         for label, n in zip(TOTALS, result):
             log("FINISHED PROCESSING, %s: %d" % (label, n))
+        if ns.sub_command == "call_variant_gvcf":
+            log("GVCF: %s" % os.path.join(ns.output_dir, "PEPPER_VARIANT.g.vcf.gz"))
     else:
         from .frontend import natural_key, write_polished_fasta, write_polished_fastq
         out = polish_output(ns.output_file)
@@ -377,7 +394,7 @@ def finish(ns: argparse.Namespace, result, t0: float) -> None:
 
 
 def _run(ns, state, device: int, distributed: bool):
-    return (run_call_variant if ns.sub_command == "call_variant" else run_polish)(ns, state, device, distributed)
+    return (run_call_variant if ns.sub_command in VARIANT_COMMANDS else run_polish)(ns, state, device, distributed)
 
 
 def _worker(rank: int, world: int, port: int, devices: list[int], ns, state, t0: float) -> None:
@@ -406,7 +423,7 @@ def _free_port() -> int:
 def execute(ns: argparse.Namespace, no_effect: list[str]) -> None:
     t0 = time.time()
     command = ns.sub_command
-    if command == "call_variant":
+    if command in VARIANT_COMMANDS:
         resolve(ns)
         log("PRESET: --%s" % ns.preset)
         for k in presets.IMAGE_KEYS + presets.CANDIDATE_KEYS:
@@ -420,7 +437,7 @@ def execute(ns: argparse.Namespace, no_effect: list[str]) -> None:
     for k in no_effect:
         log("--%s IS ACCEPTED AND HAS NO EFFECT HERE." % k)
     state = load_model(ns.model_path, MODEL_KIND[command])
-    if command == "call_variant":
+    if command in VARIANT_COMMANDS:
         os.makedirs(ns.output_dir, exist_ok=True)
     import torch.distributed as dist
     if "WORLD_SIZE" in os.environ and "RANK" in os.environ:          # launched by torchrun: run as that rank

@@ -104,6 +104,9 @@ struct pb_variant_encoder {
     cudaStream_t copy_stream = nullptr;
     cudaEvent_t copied[2] = {nullptr, nullptr};
     pb::VariantStream *vstream = nullptr;
+    // gVCF track of a streaming session (pb_variant_stream_track), set for the duration of one group's encode
+    uint32_t *track = nullptr;
+    const int64_t *track_reg = nullptr;
 };
 
 struct pb_polish_encoder {

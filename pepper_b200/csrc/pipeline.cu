@@ -73,7 +73,10 @@ extern "C" int pb_variant_call_device(pb_variant_encoder_t *enc, pb_variant_net_
 // One group of regions [g0, g1) staged into buffer set `b` on the copy stream.  Read / reference arrays keep their
 // ABSOLUTE offsets: the device base pointers are shifted back by the slice start ("virtual base"), so seq_off /
 // cigar_off / ref_off need no rebasing; only the per-read arrays are re-indexed from the group's first read.
-struct GroupView { pb_reads_t d; const pb_region_t *d_regions; const char *d_ref; std::vector<pb_region_t> h_regions; };
+struct GroupView {
+    pb_reads_t d; const pb_region_t *d_regions; const char *d_ref; std::vector<pb_region_t> h_regions;
+    std::vector<int64_t> owned_end;      // gVCF track session: each region's last owned position (pb_variant_stream_owned)
+};
 
 static int stage_group(pb_variant_encoder_t *e, int b, const pb_reads_t *h, const pb_region_t *h_regions, int64_t g0, int64_t g1,
                        const char *h_ref, GroupView &V) {
@@ -183,6 +186,12 @@ struct VariantStream {
     float enc_ms = 0.f, net_ms = 0.f;
     float enc_phase_ms[5] = {0, 0, 0, 0, 0};        // prefix, count, sites, alleles, windows — summed over the groups
     int64_t enc_launches = 0, net_launches = 0, groups = 0;
+    // gVCF track (pb_variant_stream_track): uint32 [track_cap], filled in run order; track_reg holds the running group's
+    // (track offset, owned end) per region
+    uint32_t *d_track = nullptr;
+    int64_t track_cap = 0, track_done = 0, track_need = 0;    // track_need > track_cap: a group did not fit
+    DevBuf track_reg;
+    std::vector<int64_t> h_track_reg;
 };
 }  // namespace pb
 
@@ -219,6 +228,46 @@ extern "C" int pb_variant_stream_begin(pb_variant_encoder_t *e, pb_variant_net_t
     S->enc_ms = S->net_ms = 0.f;
     for (int i = 0; i < 5; i++) S->enc_phase_ms[i] = 0.f;
     S->enc_launches = S->net_launches = S->groups = 0;
+    S->d_track = nullptr; S->track_cap = 0; S->track_done = 0; S->track_need = 0;
+    for (int b = 0; b < 2; b++) S->V[b].owned_end.clear();
+    return PB_OK;
+}
+
+// gVCF track of the session begun last: call before the first stage
+extern "C" int pb_variant_stream_track(pb_variant_encoder_t *e, int64_t capacity_positions, uint32_t *d_track) {
+    VariantStream *S;
+    PB_TRY(session(e, &S, true));
+    if (!d_track || capacity_positions < 0) { set_error("bad track"); return PB_ERR_ARG; }
+    if (S->groups > 0 || S->staged[0] || S->staged[1]) { set_error("attach the track before the first stage"); return PB_ERR_STATE; }
+    S->d_track = d_track; S->track_cap = capacity_positions; S->track_done = 0; S->track_need = 0;
+    return PB_OK;
+}
+
+// owned ends of the group staged last (one per region, absolute, inclusive): its regions' track rows are [cand_start, owned_end]
+extern "C" int pb_variant_stream_owned(pb_variant_encoder_t *e, const int64_t *h_owned_end, int64_t n) {
+    VariantStream *S;
+    PB_TRY(session(e, &S, true));
+    if (!S->d_track) { set_error("no track attached"); return PB_ERR_STATE; }
+    const int b = S->next_stage ^ 1;
+    GroupView &V = S->V[b];
+    if (!S->staged[b] || !h_owned_end || n != (int64_t) V.h_regions.size()) { set_error("owned ends do not match the staged group"); return PB_ERR_ARG; }
+    for (int64_t r = 0; r < n; r++)
+        if (h_owned_end[r] < V.h_regions[r].cand_start - 1 || h_owned_end[r] > V.h_regions[r].cand_end) {
+            set_error("region %lld: owned end %lld outside [cand_start - 1, cand_end]", (long long) r, (long long) h_owned_end[r]);
+            return PB_ERR_ARG;
+        }
+    V.owned_end.assign(h_owned_end, h_owned_end + n);
+    return PB_OK;
+}
+
+// *n_positions = track positions written so far; *n_needed = positions the groups run or refused so far needed (above the
+// capacity after a run() that returned PB_ERR_CAPACITY for the track)
+extern "C" int pb_variant_stream_track_used(pb_variant_encoder_t *e, int64_t *n_positions, int64_t *n_needed) {
+    VariantStream *S;
+    PB_TRY(session(e, &S, false));
+    if (!n_positions) { set_error("null argument"); return PB_ERR_ARG; }
+    *n_positions = S->track_done;
+    if (n_needed) *n_needed = std::max(S->track_done, S->track_need);
     return PB_OK;
 }
 
@@ -318,12 +367,36 @@ extern "C" int pb_variant_stream_run(pb_variant_encoder_t *e, pb_variant_net_t *
     GroupView &V = S->V[b];
     int64_t n_g = 0;
     const int64_t done = S->done, room = std::max<int64_t>(S->capacity - done, 0);
+    int64_t track_need = 0;
+    if (S->d_track) {
+        const int64_t nr = (int64_t) V.h_regions.size();
+        if ((int64_t) V.owned_end.size() != nr) { set_error("gVCF track session: call pb_variant_stream_owned after each stage"); return PB_ERR_STATE; }
+        S->h_track_reg.resize((size_t) 2 * nr);
+        for (int64_t r = 0; r < nr; r++) {
+            S->h_track_reg[2 * r] = S->track_done + track_need;
+            S->h_track_reg[2 * r + 1] = V.owned_end[r];
+            track_need += V.owned_end[r] - V.h_regions[r].cand_start + 1;
+        }
+        if (S->track_done + track_need > S->track_cap) {
+            S->track_need = S->track_done + track_need;
+            S->staged[b] = false; S->next_run = b ^ 1;
+            if (n_total) *n_total = done;
+            cudaStreamSynchronize(e->copy_stream);
+            set_error("gVCF track capacity %lld positions < %lld needed", (long long) S->track_cap, (long long) (S->track_done + track_need));
+            return PB_ERR_CAPACITY;
+        }
+        PB_TRY(upload(S->track_reg, S->h_track_reg.data(), sizeof(int64_t) * 2 * nr, st));
+        e->track = S->d_track; e->track_reg = S->track_reg.as<int64_t>();
+    }
     PB_CUDA(cudaEventRecord(E[0], st));
     int rc = pb_variant_encode_device(e, &V.d, V.d_regions, (int64_t) V.h_regions.size(), V.h_regions.data(), V.d_ref, 0, &S->params, room,
                                       e->p_images.as<int8_t>() + done * 33 * 26, e->p_positions.as<int64_t>() + done,
                                       e->p_depths.as<uint8_t>() + done, e->p_freqs.as<uint8_t>() + done,
                                       e->p_keys.as<char>() + done * PB_ALLELE_STRIDE, e->p_region_of.as<int32_t>() + done, nullptr, &n_g, (void *) st);
+    e->track = nullptr; e->track_reg = nullptr;
+    V.owned_end.clear();
     S->staged[b] = false; S->next_run = b ^ 1;
+    if (rc == PB_OK) S->track_done += track_need;
     if (n_total) *n_total = done + n_g;
     if (rc != PB_OK) { if (rc == PB_ERR_CAPACITY) cudaStreamSynchronize(e->copy_stream); return rc; }
     for (int i = 0; i < 5; i++) S->enc_phase_ms[i] += e->ms[i];

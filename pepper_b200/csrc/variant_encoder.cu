@@ -202,6 +202,8 @@ struct TileArgs {
     int32_t *dbg_counts;             // optional [G][3] snp, ins, del
     int32_t *tile_nsites, *tile_nev; // [n_tiles]
     RareEv *rare; unsigned long long *rare_n; unsigned long long rare_cap;
+    uint32_t *track;                 // optional gVCF track: (n_ref | n_alt << 16) per owned position
+    const int64_t *track_reg;        // [n_regions][2] track offset of cand_start, owned end (absolute, inclusive)
     VParams P;
 };
 
@@ -515,6 +517,26 @@ __global__ void __launch_bounds__(TC_THREADS, 4) k_tile_count(TileArgs A) {
         dst[0] = srcv[0];
         dst[1] = srcv[1];
         A.cov[g] = cov;
+        // gVCF track: reference / non-reference counts of an owned position over both strands, from the unclamped columns
+        // (n_ref = count(R) - I - D, n_alt = the other bases + '*' + I + D; zero over a non-ACGT reference)
+        if (A.track) {
+            const int64_t pos = lo + x, t0 = A.track_reg[2 * reg], own_end = A.track_reg[2 * reg + 1];
+            if (pos >= rg.cand_start && pos <= own_end) {
+                uint32_t v = 0;
+                if (rcls < 4) {
+                    const int ins = -((int) row[5] + row[13]), del = -((int) row[6] + row[14]), oth = -((int) row[7] + row[15]);
+                    int nalt = ins + del + oth, nref = 0;
+#pragma unroll
+                    for (int b = 0; b < 4; b++) {
+                        const int c = -((int) row[1 + b] + row[9 + b]);
+                        if (b == rcls) nref = c; else nalt += c;
+                    }
+                    nref = max(0, nref - ins - del);
+                    v = (uint32_t) min(nref, 65535) | ((uint32_t) min(max(nalt, 0), 65535) << 16);
+                }
+                A.track[t0 + pos - rg.cand_start] = v;
+            }
+        }
         const int snp = CN(C_SNP), ins = CN(C_INS), del = CN(C_DEL);
         if (A.dbg_counts) { A.dbg_counts[g * 3] = snp; A.dbg_counts[g * 3 + 1] = ins; A.dbg_counts[g * 3 + 2] = del; }
         const double c = fmax(1.0, (double) cov);
@@ -1176,6 +1198,7 @@ extern "C" int pb_variant_encode_device(pb_variant_encoder_t *e, const pb_reads_
     TA.dbg_counts = e->debug ? e->dbg.as<int32_t>() : nullptr;
     TA.tile_nsites = e->tile_nsites.as<int32_t>(); TA.tile_nev = e->tile_nev.as<int32_t>();
     TA.rare = e->rare.as<RareEv>(); TA.rare_n = reinterpret_cast<unsigned long long *>(sc + 2); TA.rare_cap = e->rare_cap;
+    TA.track = e->track; TA.track_reg = e->track_reg;
     TA.P = P;
     const size_t tc_smem = NCNT * TILE * sizeof(int32_t) + 2 * TILE;
     unsigned long long n_rare = 0;

@@ -22,6 +22,7 @@ import numpy as np
 from .abi import PRED_RECORD
 
 RECORD_BYTES = PRED_RECORD.itemsize
+GVCF_BATCH = 1 << 22        # track positions per batch of the gVCF pass: bounds its device workspace (DESIGN.md section 4)
 
 
 def shard_regions(work: np.ndarray, world: int) -> list[tuple[int, int]]:
@@ -368,16 +369,19 @@ class _RankDriver:
         return self.buffer
 
     def _run_job(self, s, claimer, groups: list[tuple[int, int]], capacity: int, source=None, stage=None, first=None,
-                 world: int | None = None) -> list[tuple[int, int]]:
+                 world: int | None = None, owned=None) -> list[tuple[int, int]]:
         """run_claimed over the job's groups: group j covers regions groups[j] = [g0, g1) of the source and is staged with region
         ids from first[j] (default g0).  From a file source (frontend._GroupSource) the fetch of a claimed group starts on the
-        source's fetch ring, one fetch per reader outstanding beside the group being run; otherwise `stage(j)` stages group j."""
+        source's fetch ring, one fetch per reader outstanding beside the group being run; otherwise `stage(j)` stages group j.
+        `owned(j)`: the owned ends of group j's regions, given to a gVCF track session after each stage."""
         from .frontend import FETCH_READERS
         request, depth = None, 1
         if source is not None:
             def stage(j):
                 g0, g1 = groups[j]
                 s.stage_device(source.take(j, g0, g1), 0, g1 - g0, g0 if first is None else first[j])
+                if owned is not None:
+                    s.owned(owned(j))
 
             def request(j):
                 source.request(j, *groups[j])
@@ -657,6 +661,10 @@ class GenomeRankPart:
         self.edges = {}
         self.meta, self.comp = b"", None
         self.phase_ms = {}
+        # gVCF: the track (device) and its groups in run order; the written lines per group after the drops
+        self.track, self.track_order, self.ref_table, self.d_ref = None, [], None, None
+        self.written, self.all_lines, self.texts = {}, None, []
+        self.track_overflow = None          # the message when this rank's gVCF track could not hold a group
 
 
 def group_table_rows(part: GenomeRankPart, n_groups: int) -> np.ndarray:
@@ -755,16 +763,21 @@ class DistributedGenomeCaller(_RankDriver):
     table and writes the files.  Returns the FindCandidates.py:185-189 totals on every rank.
 
     `capacity_bytes`: the candidate records one rank's session may hold (84 bytes each); run fails when the ranks together could
-    not run every group.  `distributed=False` runs alone at world size 1."""
+    not run every group.  `distributed=False` runs alone at world size 1.
+
+    `gvcf=True`: the sessions also fill a track of (n_ref, n_alt) per owned position (4 bytes each, `track_positions` per rank,
+    default gvcf.track_capacity); after the drops every rank builds the reference blocks and record lines of its groups on its
+    GPU (gvcf_pass) and rank 0 also writes PEPPER_VARIANT.g.vcf.gz, blocks banded by GQ // `gvcf_binsize`."""
 
     _claim_prefix = "pb_genome_claim"
 
     def __init__(self, state: dict, device: int, capacity_bytes: int, schedule: str = "dynamic", group_regions: int = 32,
-                 distributed: bool = True, caller=None):
+                 distributed: bool = True, caller=None, gvcf: bool = False, gvcf_binsize: int = 5, track_positions: int | None = None):
         from .pipeline import VariantCaller
         super().__init__(VariantCaller, state, device, schedule, group_regions, distributed, caller)
         self.device_id = device
         self.capacity = int(capacity_bytes)
+        self.gvcf, self.gvcf_binsize, self.track_positions = bool(gvcf), int(gvcf_binsize), track_positions
 
     # ---------------------------------------------------------------- per-rank work
     def run_groups(self, src, claimer, params: dict, options: dict | None = None, vcf_options: dict | None = None,
@@ -783,9 +796,27 @@ class DistributedGenomeCaller(_RankDriver):
         cap = max(1, self.capacity // RECORD_BYTES)
         t0 = time.perf_counter()
         s = self.caller.stream(params, cap)
-        segments = self._run_job(s, claimer, groups, cap, src, world=world)
+        owned = None
+        if self.gvcf:
+            from .gvcf import track_capacity
+            tcap = self.track_positions or track_capacity(sum(e - b + 1 for b, e in src.intervals), world or self.world)
+            part.track = torch.empty(max(1, int(tcap)), dtype=torch.int32, device=self.device)
+            s.track(int(tcap), part.track.data_ptr())
+            ends = owned_ends(src)
+
+            def owned(j):
+                return ends[groups[j][0]:groups[j][1]]
+        from .pipeline import TrackCapacityError
+        try:
+            segments = self._run_job(s, claimer, groups, cap, src, world=world, owned=owned)
+        except TrackCapacityError as ex:
+            # the other ranks learn of it at the first collective (call_source), so that every rank fails there alike
+            s.end()
+            part.track_overflow = str(ex)
+            return part
         n = s.end()
         part.groups = sorted(g for g, _ in segments)
+        part.track_order = [g for g, _ in segments]
         part.phase_ms["sessions"] = (time.perf_counter() - t0) * 1e3
         t0 = time.perf_counter()
         if n > 0:
@@ -814,6 +845,7 @@ class DistributedGenomeCaller(_RankDriver):
             window[:, 1] = np.where(bnd[group_of, 1] >= 0, bnd[group_of, 1] - 1, np.iinfo(np.int64).max)
             d_regions = torch.from_numpy(regions_array(table)[1]).to(dev)
             d_ref = torch.from_numpy(np.ascontiguousarray(table.ref, np.uint8)).to(dev)
+            part.ref_table, part.d_ref = table, d_ref
             text, lines = vcf_text_device(src.names, src.contig_of, cols, d_probs.value or 0, n, d_regions.data_ptr(), d_ref.data_ptr(),
                                           options or ONT_OPTIONS, vcf_options, self.device_id, window=window, on_device=True)
             part.text, part.lines = text, lines.cpu().numpy().view(VCF_LINE)
@@ -891,6 +923,7 @@ class DistributedGenomeCaller(_RankDriver):
                                    np.flatnonzero(part.line_group == g) if part.lines is not None else np.zeros(0, np.int64)]).astype(np.int64)
             if drop[g]:
                 rows = rows[1:]
+            part.written[g] = rows
             gl = all_lines[rows]
             nm = []
             for m in file_masks(gl["cls"]):
@@ -904,6 +937,7 @@ class DistributedGenomeCaller(_RankDriver):
             meta.append(np.array([g, gl.shape[0]] + nm, np.int64).tobytes())
             meta.append(None)                        # member sizes, filled in after the compression
             meta.append(group_line_table(gl).tobytes())
+        part.all_lines, part.texts = all_lines, texts
         payload = torch.empty(max(1, pay), dtype=torch.uint8, device=self.device)
         if pay:
             text_all = torch.cat(texts) if len(texts) > 1 else texts[0]
@@ -935,16 +969,19 @@ class DistributedGenomeCaller(_RankDriver):
         dist.all_gather_object(out, obj)
         return out
 
-    def _gather_bytes(self, part: GenomeRankPart) -> list | None:
-        """Every rank's meta + members into one byte GatherBuffer (one all-gather); rank 0 gets each rank's bytes."""
+    def _gather_bytes(self, part: GenomeRankPart, meta=None, comp=None) -> list | None:
+        """Every rank's meta + members (part.meta / part.comp unless given) into one byte GatherBuffer (one all-gather); rank 0
+        gets each rank's bytes."""
         import torch
-        mine = int(part.meta.shape[0]) + int(part.comp.shape[0])
+        meta = part.meta if meta is None else meta
+        comp = part.comp if comp is None else comp
+        mine = int(meta.shape[0]) + int(comp.shape[0])
         cap = max(x for x in self._all_gather_object(mine))
         buf = GatherBuffer(max(1, cap), self.world, self.rank, self.device, record=np.uint8)
         try:
             sl = buf.my_slice()
-            sl[:part.meta.shape[0]].copy_(torch.from_numpy(part.meta))
-            sl[part.meta.shape[0]:mine].copy_(part.comp)
+            sl[:meta.shape[0]].copy_(torch.from_numpy(meta))
+            sl[meta.shape[0]:mine].copy_(comp)
             buf.gather(mine)
             torch.cuda.synchronize(self.device)
             if self.rank != 0:
@@ -957,6 +994,7 @@ class DistributedGenomeCaller(_RankDriver):
     def call_genome(self, bam: str, fasta: str, out_dir: str, sample_name: str, region: str | None = None, exclude=(),
                     params: dict | None = None, options: dict | None = None, vcf_options: dict | None = None,
                     interval_size: int = 100_000, gpu_inflate: bool = True) -> tuple:
+        """Rank 0 writes the five PEPPER_VARIANT_*.vcf.gz (and, with gvcf=True, PEPPER_VARIANT.g.vcf.gz) under out_dir."""
         from .frontend import VariantGenomeSource
         from .synth import ont_params
         params = params or ont_params()
@@ -976,7 +1014,13 @@ class DistributedGenomeCaller(_RankDriver):
         groups = src.groups(self.group_regions)
         part = self.run_groups(src, self._claimer(len(groups), src.group_work(groups)), params, options, vcf_options)
         t0 = time.perf_counter()
-        held = self._all_gather_object(part.held)
+        held = self._all_gather_object((part.held, part.track_overflow))
+        over = [(r, m) for r, (_, m) in enumerate(held) if m is not None]
+        if over:
+            from .pipeline import TrackCapacityError
+            from .abi import PB_ERR_CAPACITY
+            raise TrackCapacityError("rank %d: %s" % over[0], PB_ERR_CAPACITY)
+        held = [h for h, _ in held]
         held = np.concatenate(held) if held else np.zeros(0, PRED_RECORD)
         part.phase_ms["edge_exchange"] = (time.perf_counter() - t0) * 1e3
         self.edge_pass(part, src, held, options, vcf_options)
@@ -995,10 +1039,181 @@ class DistributedGenomeCaller(_RankDriver):
             write_vcfs_from_parts(out_dir, sample_name, src.fasta_contigs(), src.names,
                                   [int(src.contig_of[g0]) for g0, _ in groups], parts)
         part.phase_ms["write"] = (time.perf_counter() - t0) * 1e3
+        if self.gvcf:
+            self._call_gvcf(part, src, out_dir, sample_name)
         part.phase_ms["groups"] = len(part.groups)
         self.phase_ms = {k: round(v, 2) for k, v in part.phase_ms.items()}
         self.payload_bytes, self.member_bytes = part.payload_bytes, int(part.comp.shape[0])
         return totals
+
+    # ---------------------------------------------------------------- gVCF
+    def _call_gvcf(self, part: GenomeRankPart, src, out_dir: str, sample_name: str):
+        import time
+        import torch
+        from .gvcf import parse_gvcf_bytes, write_gvcf_from_parts
+        groups = src.groups(self.group_regions)
+        t0 = time.perf_counter()
+        # each group's largest written record end (-1: none), then the running maximum of the earlier groups of its contig
+        mine = np.full(len(groups), -1, np.int64)
+        for g, rows in part.written.items():
+            if rows.shape[0]:
+                mine[g] = int((part.all_lines["pos"][rows] + part.all_lines["ref_len"][rows]).max())
+        ends = np.maximum.reduce(self._all_gather_object(mine))
+        part.phase_ms["gvcf_exchange"] = (time.perf_counter() - t0) * 1e3
+        meta, comp = self.gvcf_pass(part, src, mask_until(ends, [int(src.contig_of[g0]) for g0, _ in groups]))
+        t0 = time.perf_counter()
+        # the members are on the host: one rank keeps them there, several all-gather them through their GPUs
+        got = [np.concatenate([meta, comp])] if self.world == 1 else self._gather_bytes(part, meta, torch.from_numpy(comp))
+        part.phase_ms["gvcf_gather"] = (time.perf_counter() - t0) * 1e3
+        t0 = time.perf_counter()
+        if got is not None:
+            parts = {}
+            for data in got:
+                parts.update(parse_gvcf_bytes(data))
+            write_gvcf_from_parts(out_dir, sample_name, src.fasta_contigs(), src.names, [int(src.contig_of[g0]) for g0, _ in groups],
+                                  parts)
+        part.phase_ms["gvcf_write"] = (time.perf_counter() - t0) * 1e3
+
+    def gvcf_pass(self, part: GenomeRankPart, src, until: np.ndarray, batch_positions: int = GVCF_BATCH):
+        """This rank's gVCF lines, in batches of whole groups of about `batch_positions` track positions (run order): per batch,
+        the reference blocks of its track slice (positions inside a written record's span, or before `until[g]` of group g, are
+        masked) and its written FULL lines with the <*> allele, merged by position per group, laid out on the device and
+        compressed to BGZF members, which go to the host before the next batch.  Device memory beyond the track is bounded by
+        the batch.  Returns (meta bytes, members) for the byte gather, both host arrays."""
+        import time
+        import torch
+        from .gvcf import GVCF_SEGMENT, GVCF_LINE, gvcf_blocks_device, gvcf_records_device
+        from .vcf import VCF_LINE, member_cuts, gather_lines_device, bgzf_compress_device
+        groups = src.groups(self.group_regions)
+        ends = owned_ends(src)
+        regs = [r for g in part.track_order for r in range(*groups[g])]
+        if part.ref_table is None and regs:
+            part.ref_table = src.table(regs)
+            part.d_ref = torch.from_numpy(np.ascontiguousarray(part.ref_table.ref, np.uint8)).to(self.device)
+        gstart = np.array([(int(src.contig_of[g0]) << 40) | src.intervals[g0][0] for g0, _ in groups], np.int64)
+        text_all = None
+        if part.texts:
+            text_all = torch.cat(part.texts) if len(part.texts) > 1 else part.texts[0]
+        ms = dict(gvcf_blocks=0.0, gvcf_records=0.0, gvcf_merge_host=0.0, gvcf_layout=0.0, gvcf_compress=0.0)
+        stats = dict(track_bytes=0, block_lines=0, record_lines=0, payload_bytes=0, compressed_bytes=0)
+        heads, comps = [], []
+
+        def flush(batch, t0):
+            n = sum(t for _, t in batch)
+            seg, masks, rec_rows, toff_g, t = [], [], [], {}, 0
+            for g, _ in batch:
+                g0, g1 = groups[g]
+                p0, p1 = src.intervals[g0][0], int(ends[g1 - 1])
+                toff_g[g] = t
+                for r in range(g0, g1):
+                    s0 = src.intervals[r][0]
+                    row = part.ref_table.table[r]
+                    seg.append((t, s0, int(ends[r]) - s0 + 1, int(row[4]) + s0 - int(row[0]), int(src.contig_of[r]), 0))
+                    t += int(ends[r]) - s0 + 1
+                rows = part.written.get(g, np.zeros(0, np.int64))
+                rec_rows.append(rows)
+                if until[g] > p0:
+                    masks.append(np.array([[toff_g[g], toff_g[g] + min(int(until[g]), p1 + 1) - p0]], np.int64))
+                if rows.shape[0]:
+                    pos = part.all_lines["pos"][rows].astype(np.int64)
+                    end = np.minimum(pos + part.all_lines["ref_len"][rows], p1 + 1)
+                    masks.append(np.stack([toff_g[g] + pos - p0, toff_g[g] + end - p0], 1))
+            seg = np.array(seg, GVCF_SEGMENT)
+            masks = np.concatenate(masks) if masks else np.zeros((0, 2), np.int64)
+            t1 = time.perf_counter()
+            btext, blines = gvcf_blocks_device(part.track[t0:t0 + n], n, seg, masks, part.d_ref.data_ptr(), src.names,
+                                               self.gvcf_binsize, self.device_id)
+            t2 = time.perf_counter()
+            rows = np.concatenate(rec_rows)
+            if rows.shape[0]:
+                rtext, rlines = gvcf_records_device(text_all, part.all_lines[rows], self.device_id)
+            else:
+                rtext, rlines = None, np.zeros(0, VCF_LINE)
+            torch.cuda.synchronize(self.device)
+            t3 = time.perf_counter()
+            # merge: each line's group (blocks by position: the last group of the contig starting at or before it; records by
+            # their rows), then position order inside each group, laid out back to back
+            nb = blines.shape[0]
+            lines = np.concatenate([blines, rlines])
+            bgroup = np.searchsorted(gstart, (blines["contig"].astype(np.int64) << 40) | blines["pos"], side="right") - 1
+            rgroup = np.repeat(np.array([g for g, _ in batch], np.int64), [r.shape[0] for r in rec_rows])
+            lgroup = np.concatenate([bgroup, rgroup]).astype(np.int64)
+            order = np.lexsort((lines["pos"], lgroup))
+            ln = lines["text_len"].astype(np.int64)[order]
+            dst = np.concatenate([[0], np.cumsum(ln)[:-1]]) if order.shape[0] else np.zeros(0, np.int64)
+            ids = sorted(g for g, _ in batch)
+            bounds = np.searchsorted(lgroup[order], np.array(ids + [np.iinfo(np.int64).max]), side="left")
+            member_off, pay, batch_heads = [0], 0, []
+            for i, g in enumerate(ids):
+                sel = order[bounds[i]:bounds[i + 1]]
+                nbytes = int(ln[bounds[i]:bounds[i + 1]].sum())
+                cuts = member_cuts(nbytes)
+                member_off.extend((pay + np.cumsum(cuts)).tolist())
+                pay += nbytes
+                gl = np.zeros(sel.shape[0], GVCF_LINE)
+                gl["pos"], gl["end"], gl["text_len"] = lines["pos"][sel], lines["pos"][sel] + lines["ref_len"][sel], lines["text_len"][sel]
+                batch_heads.append((g, gl, cuts))
+            t4 = time.perf_counter()
+            payload = torch.empty(max(1, pay), dtype=torch.uint8, device=self.device)
+            isb = order < nb
+            for mine, text, tab, shift in ((isb, btext, blines, 0), (~isb, rtext, rlines, nb)):
+                if mine.any():
+                    d_lines = torch.from_numpy(np.ascontiguousarray(tab).view(np.uint8).reshape(-1)).to(self.device)
+                    gather_lines_device(text, d_lines, order[mine] - shift, dst[mine], payload, self.device_id)
+            torch.cuda.synchronize(self.device)
+            t5 = time.perf_counter()
+            comp, sizes = bgzf_compress_device(payload, np.array(member_off, np.int64), self.device_id)
+            comps.append(comp.cpu().numpy())
+            t6 = time.perf_counter()
+            k = 0
+            for g, gl, cuts in batch_heads:
+                heads.append((g, gl, cuts, sizes[k:k + cuts.shape[0]]))
+                k += cuts.shape[0]
+            ms["gvcf_blocks"] += (t2 - t1) * 1e3; ms["gvcf_records"] += (t3 - t2) * 1e3; ms["gvcf_merge_host"] += (t4 - t3) * 1e3
+            ms["gvcf_layout"] += (t5 - t4) * 1e3; ms["gvcf_compress"] += (t6 - t5) * 1e3
+            stats["track_bytes"] += 4 * n; stats["block_lines"] += nb; stats["record_lines"] += int(rlines.shape[0])
+            stats["payload_bytes"] += pay; stats["compressed_bytes"] += int(comps[-1].shape[0])
+
+        batch, t0, tb = [], 0, 0
+        for g in part.track_order:
+            g0, g1 = groups[g]
+            n = int(ends[g1 - 1]) - src.intervals[g0][0] + 1
+            batch.append((g, n))
+            tb += n
+            if tb >= batch_positions:
+                flush(batch, t0)
+                t0, batch, tb = t0 + tb, [], 0
+        if batch:
+            flush(batch, t0)
+        meta = []
+        for g, gl, cuts, sz in heads:
+            meta += [np.array([g, gl.shape[0], cuts.shape[0]], np.int64).tobytes(), cuts.astype(np.int64).tobytes(),
+                     sz.astype(np.int64).tobytes(), gl.tobytes()]
+        body = b"".join(meta)
+        meta = np.frombuffer(np.array([16 + len(body), len(heads)], np.int64).tobytes() + body, np.uint8).copy()
+        part.phase_ms.update(ms)
+        self.gvcf_stats = stats
+        return meta, (np.concatenate(comps) if comps else np.zeros(0, np.uint8))
+
+
+def owned_ends(src) -> np.ndarray:
+    """The last position each interval owns: e - 1 for (s, e), e for the last interval of its contig's span."""
+    ends = np.array([e - 1 for _, e in src.intervals], np.int64)
+    first = np.array(src._first, np.int64)
+    ends[(first[1:] - 1)[np.diff(first) > 0]] += 1
+    return ends
+
+
+def mask_until(ends: np.ndarray, group_contig: list[int]) -> np.ndarray:
+    """Per group: the largest written record end (exclusive) of the earlier groups of its contig (-1 when none)."""
+    out = np.full(len(group_contig), -1, np.int64)
+    run, prev = -1, None
+    for g, c in enumerate(group_contig):
+        if c != prev:
+            run, prev = -1, c
+        out[g] = run
+        run = max(run, int(ends[g]))
+    return out
 
 
 def _device_column(ptr: int, shape: tuple, typestr: str, device):

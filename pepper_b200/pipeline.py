@@ -73,6 +73,9 @@ def _bind_calls(L):
     L.pb_variant_stream_stats.argtypes = [vp, vp, vp, C.POINTER(C.c_int64)]
     L.pb_variant_stream_columns.argtypes = [vp, C.POINTER(PbCandidateColumns), C.POINTER(vp), C.POINTER(vp)]
     L.pb_variant_stream_fetch.argtypes = [vp, C.c_int64, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.pb_variant_stream_track.argtypes = [vp, C.c_int64, vp]
+    L.pb_variant_stream_owned.argtypes = [vp, vp, C.c_int64]
+    L.pb_variant_stream_track_used.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.pb_polish_call_host.argtypes = [vp, vp, C.POINTER(PbReads), C.POINTER(PbRegion), C.c_int64, C.c_int64, vp, vp, vp, vp,
                                       vp, vp, C.POINTER(C.c_int64), vp]
     L.pb_polish_call_device.argtypes = [vp, vp, C.POINTER(PbReads), vp, C.c_int64, C.POINTER(PbRegion), C.c_int64, vp, vp,
@@ -208,6 +211,10 @@ class VariantCaller:
         return VariantStream(self, params, capacity, d_records, stream)
 
 
+class TrackCapacityError(_lib.PepperB200Error):
+    """A streaming session's gVCF track could not hold the next group (rc PB_ERR_CAPACITY)."""
+
+
 class VariantStream:
     """One streaming session of a VariantCaller: region GROUPS are staged and run one after the other, the candidates
     accumulate on the device, the network runs over whole 9,472-candidate chunks as they fill.
@@ -238,9 +245,33 @@ class VariantStream:
         _lib.check(self.L.pb_variant_stream_stage_device(self.c.enc.h, C.byref(dreads.struct), dreads.h_regions, g0, g1,
                                                          C.c_void_p(dreads.d_ref), region_id0), "pb_variant_stream_stage_device")
 
+    def track(self, capacity_positions: int, d_track: int):
+        """Attaches a gVCF track (pb_variant_stream_track): uint32 device buffer [capacity_positions]; stage_device then takes
+        each group's owned ends."""
+        _lib.check(self.L.pb_variant_stream_track(self.c.enc.h, int(capacity_positions), C.c_void_p(d_track)), "pb_variant_stream_track")
+        self.track_capacity = int(capacity_positions)
+
+    def owned(self, owned_end):
+        """The owned ends of the group staged last (pb_variant_stream_owned)."""
+        a = np.ascontiguousarray(owned_end, np.int64)
+        _lib.check(self.L.pb_variant_stream_owned(self.c.enc.h, a.ctypes.data, a.shape[0]), "pb_variant_stream_owned")
+
+    def track_used(self) -> int:
+        return self._track_counts()[0]
+
+    def _track_counts(self) -> tuple[int, int]:
+        n, need = C.c_int64(0), C.c_int64(0)
+        _lib.check(self.L.pb_variant_stream_track_used(self.c.enc.h, C.byref(n), C.byref(need)), "pb_variant_stream_track_used")
+        return int(n.value), int(need.value)
+
     def run(self, flush: bool = False) -> int:
         n = C.c_int64(0)
         rc = self.L.pb_variant_stream_run(self.c.enc.h, self.c.net.h, int(flush), C.byref(n))
+        if rc == PB_ERR_CAPACITY and getattr(self, "track_capacity", None) is not None:
+            used, need = self._track_counts()
+            if need > self.track_capacity:
+                raise TrackCapacityError("gVCF track capacity %d positions too small (need >= %d so far)"
+                                         % (self.track_capacity, need), rc)
         if rc == PB_ERR_CAPACITY:
             raise _lib.PepperB200Error("stream capacity %d too small (need >= %d so far)" % (self.capacity, n.value), rc)
         _lib.check(rc, "pb_variant_stream_run")

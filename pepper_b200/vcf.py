@@ -526,40 +526,50 @@ def write_vcfs_from_parts(out_dir: str, sample_name: str, fasta_contigs: list[tu
     same lines, up to the DEFLATE bytes of the members."""
     import os
     from concurrent.futures import ThreadPoolExecutor
-    from .synth_files import BGZF_EOF
     os.makedirs(out_dir, exist_ok=True)
     head = vcf_header(sample_name, fasta_contigs).encode()
     lex = {c: i for i, c in enumerate(sorted(range(len(names)), key=lambda i: names[i]))}
     order = sorted(parts, key=lambda g: (lex[group_contig[g]], g))
     depth = vcf_csi_depth(fasta_contigs, names)
     with ThreadPoolExecutor(max_workers=8) as pool:
-        hgz, hu, hc = _bgzf(head, pool, 1)
-        hgz = hgz[:-len(BGZF_EOF)]
         for f, name in enumerate(VCF_FILES):
-            chunks, blk_u, blk_c = [hgz], [hu], [hc[:-1]]
-            u, c = len(head), len(hgz)
-            tids, beg, end, ulen, seen = [], [], [], [], {}
+            pieces = []
             for g in order:
                 p = parts[g]
                 sel = p.lines[file_masks(p.lines["cls"])[f]]
-                if p.usizes[f].shape[0]:
-                    blk_u.append(u + np.concatenate([[0], np.cumsum(p.usizes[f])[:-1]]))
-                    blk_c.append(c + np.concatenate([[0], np.cumsum(p.csizes[f])[:-1]]))
-                    chunks.append(p.data[f])
-                    u += int(p.usizes[f].sum()); c += int(p.csizes[f].sum())
-                if sel.shape[0]:
-                    tids.append(np.full(sel.shape[0], seen.setdefault(group_contig[g], len(seen)), np.int64))
-                    beg.append(sel["pos"]); end.append(sel["pos"] + sel["ref_len"]); ulen.append(sel["text_len"].astype(np.int64))
-            path = os.path.join(out_dir, name + ".vcf.gz")
-            with open(path, "wb") as fh:
-                fh.write(b"".join(chunks) + BGZF_EOF)
-            cat = (lambda a, dt: np.concatenate(a) if a else np.zeros(0, dt))     # noqa: E731
-            ul = cat(ulen, np.int64)
-            us = len(head) + np.concatenate([[0], np.cumsum(ul)])
-            tbi = _tabix([names[k] for k in seen], cat(tids, np.int64), cat(beg, np.int64), cat(end, np.int64), us[:-1], us[1:],
-                         np.concatenate(blk_u), np.concatenate(blk_c), c, u, depth)
-            with open(path + (".tbi" if depth is None else ".csi"), "wb") as fh:
-                fh.write(_bgzf(tbi, pool)[0])
+                pieces.append((group_contig[g], p.usizes[f], p.csizes[f], p.data[f], sel["pos"], sel["pos"] + sel["ref_len"],
+                               sel["text_len"]))
+            write_indexed_members(os.path.join(out_dir, name + ".vcf.gz"), head, pieces, names, depth, pool)
+
+
+def write_indexed_members(path: str, head: bytes, pieces: list, names: list[str], depth: int | None, pool) -> None:
+    """One bgzipped file and its index from BGZF members compressed elsewhere: the header as its own members, then each piece
+    (contig id, member payload sizes, member compressed sizes, member bytes, line begins, line ends, line lengths) in file
+    order, then the EOF block; the .tbi (or, with `depth`, the .csi) indexes each line over [begin, end)."""
+    from .synth_files import BGZF_EOF
+    hgz, hu, hc = _bgzf(head, pool, 1)
+    hgz = hgz[:-len(BGZF_EOF)]
+    chunks, blk_u, blk_c = [hgz], [hu], [hc[:-1]]
+    u, c = len(head), len(hgz)
+    tids, beg, end, ulen, seen = [], [], [], [], {}
+    for contig, usizes, csizes, data, b, e, tl in pieces:
+        if usizes.shape[0]:
+            blk_u.append(u + np.concatenate([[0], np.cumsum(usizes)[:-1]]))
+            blk_c.append(c + np.concatenate([[0], np.cumsum(csizes)[:-1]]))
+            chunks.append(data)
+            u += int(usizes.sum()); c += int(csizes.sum())
+        if b.shape[0]:
+            tids.append(np.full(b.shape[0], seen.setdefault(contig, len(seen)), np.int64))
+            beg.append(b); end.append(e); ulen.append(tl.astype(np.int64))
+    with open(path, "wb") as fh:
+        fh.write(b"".join(chunks) + BGZF_EOF)
+    cat = (lambda a, dt: np.concatenate(a) if a else np.zeros(0, dt))     # noqa: E731
+    ul = cat(ulen, np.int64)
+    us = len(head) + np.concatenate([[0], np.cumsum(ul)])
+    tbi = _tabix([names[k] for k in seen], cat(tids, np.int64), cat(beg, np.int64), cat(end, np.int64), us[:-1], us[1:],
+                 np.concatenate(blk_u), np.concatenate(blk_c), c, u, depth)
+    with open(path + (".tbi" if depth is None else ".csi"), "wb") as fh:
+        fh.write(_bgzf(tbi, pool)[0])
 
 
 def bgzf_compress_host(payload: np.ndarray, member_off: np.ndarray) -> tuple[bytes, np.ndarray]:

@@ -9,7 +9,12 @@ after decompression.  Prints one JSON line.  Default size: 64 Mb in total (chr20
 Under torchrun the ranks run dist.DistributedGenomeCaller on the same job instead (rank 0 simulates the files into a directory
 every rank reads): rank 0 prints the JSON line with each stage's maximum over the ranks, and `verified` compares the decompressed
 files with a one-GPU call_genome run on rank 0 outside the timed window.
-    torchrun --nproc-per-node N scripts/bench_call_genome.py [--total-mb 64]"""
+    torchrun --nproc-per-node N scripts/bench_call_genome.py [--total-mb 64]
+
+With --gvcf, one GPU runs dist.DistributedGenomeCaller over the job with and without the gVCF, alternating (--repeats each), and
+reports both walls, the gVCF stages, the track bytes, the block and record lines and the compressed gVCF size; `verified` says
+the five VCFs of every gVCF run equal those of the run without it after decompression.
+    python scripts/bench_call_genome.py --gvcf [--total-mb 64] [--repeats 3]"""
 import argparse
 import gzip
 import json
@@ -34,6 +39,8 @@ def main():
     ap.add_argument("--total-mb", type=float, default=64.0)
     ap.add_argument("--coverage", type=float, default=20.0)
     ap.add_argument("--seed", type=int, default=41)
+    ap.add_argument("--gvcf", action="store_true")
+    ap.add_argument("--repeats", type=int, default=3)
     a = ap.parse_args()
     from oracle import nets
     from pepper_b200 import synth, synth_files, _lib
@@ -64,6 +71,8 @@ def main():
     bases = sum(n for _, n in lens)
     state = nets.make_variant_weights(0)
     params = synth.ont_params()
+    if a.gvcf:
+        return bench_gvcf(a, bam, fa, tmp, bases, state, params, card)
     with VariantFromFiles(bam, fa, state) as vf:
         vf.call_genome(os.path.join(tmp, "warm"), "sample", region="chr2:0-2000000", params=params)   # module load, first launches
         log("warm-up done")
@@ -104,6 +113,68 @@ def main():
                           writer=round(t_write * 1e3, 2)),
         verified=bool(same), card=card, gen_seconds=round(gen_s, 1),
         notes="one GPU: no gather (gather ms null); vcf_pass = host wall around the synchronous device VCF pass, uploads included")))
+
+
+def bench_gvcf(a, bam, fa, tmp, bases, state, params, card):
+    import numpy as np
+    import torch
+    from pepper_b200.cli import variant_capacity
+    from pepper_b200.dist import DistributedGenomeCaller
+    from pepper_b200.frontend import VariantGenomeSource
+    from pepper_b200.pipeline import VariantCaller
+    from pepper_b200.vcf import VCF_FILES
+    caller = VariantCaller(state, 0)
+    src = VariantGenomeSource(bam, fa, int(params["min_snp_baseq"]))
+    cap = 4 * variant_capacity(bases, 1)        # room for the seeded random weights' candidates: no restart inside a timed run
+    walls, phases, stats, outs = {False: [], True: []}, [], None, {}
+
+    peaks = {False: 0, True: 0}
+
+    def run(gvcf, out):
+        dgc = DistributedGenomeCaller(None, 0, cap, "dynamic", distributed=False, caller=caller, gvcf=gvcf)
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats()
+        t0 = time.perf_counter()
+        dgc.call_source(src, out, "sample", params)
+        torch.cuda.synchronize()
+        w = time.perf_counter() - t0
+        peaks[gvcf] = max(peaks[gvcf], int(torch.cuda.max_memory_allocated()))
+        ph, st = dgc.phase_ms, getattr(dgc, "gvcf_stats", None)
+        dgc.close()
+        return w, ph, st
+    try:
+        run(False, os.path.join(tmp, "warm"))
+        run(True, os.path.join(tmp, "warm_g"))
+        log("warm-up done")
+        for k in range(a.repeats):
+            for gvcf in (False, True):
+                out = os.path.join(tmp, "g%d_%d" % (k, gvcf))
+                w, ph, st = run(gvcf, out)
+                walls[gvcf].append(w)
+                outs.setdefault(gvcf, []).append(out)
+                if gvcf:
+                    phases.append(ph); stats = st
+                log("run %d gvcf=%s: %.2f s" % (k, gvcf, w))
+    finally:
+        src.close()
+        caller.close()
+    files = lambda d: [gzip.decompress(open(os.path.join(d, f + ".vcf.gz"), "rb").read()) for f in VCF_FILES]   # noqa: E731
+    want = files(outs[False][0])
+    same = all(files(d) == want for d in outs[False] + outs[True])
+    g = os.path.join(outs[True][-1], "PEPPER_VARIANT.g.vcf.gz")
+    med = lambda x: round(float(np.median(x)), 3)                               # noqa: E731
+    stage = lambda k: round(float(np.median([p.get(k, 0.0) for p in phases])), 2)   # noqa: E731
+    print(json.dumps(dict(
+        metric="call_genome_gvcf", value=bases / med(walls[True]), unit="genomic bases/s", genomic_bases=bases, coverage=a.coverage,
+        wall_s=dict(without_gvcf=[round(x, 3) for x in walls[False]], with_gvcf=[round(x, 3) for x in walls[True]],
+                    median_without=med(walls[False]), median_with=med(walls[True])),
+        gvcf_stage_ms=dict(exchange=stage("gvcf_exchange"), blocks_device=stage("gvcf_blocks"), records_device=stage("gvcf_records"),
+                           merge_host=stage("gvcf_merge_host"), layout_device=stage("gvcf_layout"), compression=stage("gvcf_compress"),
+                           gather=stage("gvcf_gather"), index_and_write=stage("gvcf_write")),
+        track_bytes=stats["track_bytes"], block_lines=stats["block_lines"], record_lines=stats["record_lines"],
+        gvcf_payload_bytes=stats["payload_bytes"], gvcf_file_bytes=os.path.getsize(g), verified=bool(same), card=card,
+        peak_torch_allocated_bytes=dict(without_gvcf=peaks[False], with_gvcf=peaks[True]),     # the library's own buffers not included
+        notes="medians over alternating runs in one process; stage times are host walls around synchronous device work")))
 
 
 def main_distributed():

@@ -23,5 +23,6 @@ for tool in memcheck racecheck; do
     run stitch_sink $tool tests/test_polish_assembly_gpu.py -k "stitch_sink"                           # k_stitch_sink
     run vcf $tool tests/test_genome_vcf_gpu.py -k "vcf_host"                                         # k_site_sizes, k_site_write
     run bgzf_deflate $tool tests/test_genome_dist_gpu.py -k "compressor"                             # k_bgzf_deflate, k_bgzf_compact
+    run gvcf $tool tests/test_gvcf_gpu.py -k "block_pass and 1 or track_matches"                    # k_gvcf_*, k_tile_count track store
 done
 cat "$OUT/sanitizer_summary.txt"
