@@ -465,6 +465,10 @@ int pb_test_tc_gemm_ex(int M, int N, int epi, int K0, const float *h_A0, int lo0
  * (NULL = not written): h_y_f32 [M][33][512]; h_y_hi / h_y_lo [ceil(M / 128)][33][16][4096]; h_c_final [2][256][M].      */
 int pb_test_variant_lstm_layer(pb_variant_net_t *net, int layer, int M, const void *h_x, int lo_x, int lo_h, int persist,
                                int poison, float *h_y_f32, uint16_t *h_y_hi, uint16_t *h_y_lo, float *h_c_final);
+/* diagnostics: the encoder LSTM layer of mode 2, which hands the decoder its h as int8 slices (k_lstm_layer_enc).  h_x: int8
+ * images [M][33][26].  h_q: int8 [2][ceil(M / 128)][33][8][128][64], the slice tiles as the layer writes them (slice 1, then
+ * slice 0).  poison: that buffer is filled with 0xff bytes first, which padding rows keep. */
+int pb_test_variant_enc_q8(pb_variant_net_t *net, int M, const int8_t *h_x, int poison, int8_t *h_q);
 /* diagnostics: the int8-slice decoder LSTM layer of mode 2 (k_lstm_layer_q8).  h_x: fp32 [M][33][512], quantized on the host
  * to the slices the encoder would write.  persist 0 = one launch per step.  Outputs (each may be NULL): y_f32 [M][33][512];
  * h_q: the layer's own h slices, 2 x ceil(M / 128) x 33 x 8 x 8192 bytes (slice 1, then slice 0; tc_gemm.cuh QSeq layout);

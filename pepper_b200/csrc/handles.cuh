@@ -7,7 +7,8 @@ namespace pb {
 struct VariantStream;      // streaming session state (pipeline.cu)
 // network layers (nets_tc.cu): weights as 16-bit hi/lo tile images + the fp32 bias; per-chunk tiled operands
 // `scale`: the power of two s the tiles hold s W in (max |s W| in (2^14, 2^15]); the epilogues multiply by 1 / s
-struct TcRnn { DevBuf w_hi, w_lo, bias; int nkt_x = 0, nkt_h = 0; float scale = 1.f; };
+// wh_hi / wh_lo (the variant encoder only): the same weights in 128-row half tiles for k_lstm_layer_enc
+struct TcRnn { DevBuf w_hi, w_lo, wh_hi, wh_lo, bias; int nkt_x = 0, nkt_h = 0; float scale = 1.f; };
 struct TcLin { DevBuf w_hi, w_lo, bias; int nkt = 0; float scale = 1.f; };
 // a weight matrix on int8 slices (mode 2: the decoder layer, tc_gemm.cuh k_lstm_layer_q8, and linear_1, k_gemm_q8): the two
 // slices of round(sw_n W[n][k]), sw_n = 32512 / max_k |W[n][k]| over the row's K (the decoder: [W_ih | W_hh]), as
@@ -72,7 +73,7 @@ struct SinkArgs {
 int polish_sink(SinkArgs A, DevBuf &counts, DevBuf &offsets, cudaStream_t st, DevBuf *ev = nullptr);
 struct PolishStream;       // streaming polish session state (pipeline.cu)
 void polish_stream_free(PolishStream *S);
-int tc_upload_rnn(TcRnn &T, const float *Wp, const float *bias, int K0, int K0p_src, int H, int Kp_src);
+int tc_upload_rnn(TcRnn &T, const float *Wp, const float *bias, int K0, int K0p_src, int H, int Kp_src, bool half_tiles = false);
 int tc_upload_lin(TcLin &T, const float *w, const float *bias, int N, int K);
 int tc_upload_rnn_q8(TcQ8 &T, const float *Wp, int K0, int K0p_src, int H, int Kp_src);
 int tc_upload_q8(TcQ8 &T, const float *W, int N, int K, bool a_quant);

@@ -126,7 +126,7 @@ extern "C" int pb_variant_net_create(pb_variant_net_t **out, int device, const f
     for (int d = 0; d < 2; d++) {
         const PackedRnn pe = pack_lstm(P[4 * d + 0], P[4 * d + 1], P[4 * d + 2], P[4 * d + 3], 26, VH);
         const PackedRnn pd = pack_lstm(P[8 + 4 * d + 0], P[8 + 4 * d + 1], P[8 + 4 * d + 2], P[8 + 4 * d + 3], 512, VH);
-        PB_TRY(tc_upload_rnn(T.enc[d], pe.W.data(), pe.bias.data(), pe.K0, pe.K0p, VH, pe.Kp));
+        PB_TRY(tc_upload_rnn(T.enc[d], pe.W.data(), pe.bias.data(), pe.K0, pe.K0p, VH, pe.Kp, true));
         PB_TRY(tc_upload_rnn(T.dec[d], pd.W.data(), pd.bias.data(), pd.K0, pd.K0p, VH, pd.Kp));
         PB_TRY(tc_upload_rnn_q8(T.decq[d], pd.W.data(), pd.K0, pd.K0p, VH, pd.Kp));
     }
@@ -165,7 +165,7 @@ extern "C" int pb_variant_net_destroy(pb_variant_net_t *N) {
     TcVariant &T = N->tc;
     for (int d = 0; d < 2; d++) {
         TcRnn *rnn[] = {&T.enc[d], &T.dec[d]};
-        for (auto *r : rnn) { r->w_hi.release(); r->w_lo.release(); r->bias.release(); }
+        for (auto *r : rnn) { r->w_hi.release(); r->w_lo.release(); r->wh_hi.release(); r->wh_lo.release(); r->bias.release(); }
         T.decq[d].w1.release(); T.decq[d].w0.release(); T.decq[d].col_scale.release();
     }
     T.lin1q.w1.release(); T.lin1q.w0.release(); T.lin1q.col_scale.release();

@@ -63,8 +63,10 @@ static float pow2_scale(const float *w, size_t n) {
 }
 
 // weights of one RNN direction, packed rows 4j+g (nets.cu pack_lstm / pack_gru) with K = [x | pad32 | h]; x-part and h-part
-// share one scale
-int tc_upload_rnn(TcRnn &T, const float *Wp /* [4H][Kp_src] */, const float *bias /* [4H] */, int K0, int K0p_src, int H, int Kp_src) {
+// share one scale.  half_tiles: also in 128-row tiles (wh_hi / wh_lo), whose k-tiles are the single 8 KB pieces that
+// k_lstm_layer_enc's ring stages take (a 128-row half of a 256-row tile is 4 pieces of 2 KB, one per 8-k chunk)
+int tc_upload_rnn(TcRnn &T, const float *Wp /* [4H][Kp_src] */, const float *bias /* [4H] */, int K0, int K0p_src, int H, int Kp_src,
+                  bool half_tiles) {
     const int K0p = (K0 + 31) / 32 * 32;
     const int Kp = K0p + H;
     std::vector<float> W((size_t) 4 * H * Kp, 0.f);
@@ -78,7 +80,10 @@ int tc_upload_rnn(TcRnn &T, const float *Wp /* [4H][Kp_src] */, const float *bia
     tile_matrix(W.data(), 4 * H, Kp, 4 * H, Kp, hi, lo, 256);
     T.nkt_x = K0p / 32; T.nkt_h = H / 32;
     PB_TRY(upload(T.bias, bias, sizeof(float) * 4 * H, 0));
-    return upload_tiles(T.w_hi, T.w_lo, hi, lo);
+    PB_TRY(upload_tiles(T.w_hi, T.w_lo, hi, lo));
+    if (!half_tiles) return PB_OK;
+    tile_matrix(W.data(), 4 * H, Kp, 4 * H, Kp, hi, lo, 128);
+    return upload_tiles(T.wh_hi, T.wh_lo, hi, lo);
 }
 int tc_upload_lin(TcLin &T, const float *w, const float *bias, int N, int K) {
     T.scale = pow2_scale(w, (size_t) N * K);
@@ -220,9 +225,11 @@ extern "C" int pb_lstm_trace_copy(uint64_t *host, int64_t n_words) {
 // One bidirectional LSTM layer of the variant network over its 33 steps, reading T.img_op (layer 0) or T.yenc (layer 1)
 // and writing T.yenc / T.ydec (+ the optional fp32 copy y_f32 [B][33][512]); the cell state ends in T.c.  lo_x / lo_h:
 // the a_lo x w_hi product of the x-part / h-part runs (the int8 images of layer 0 have no lo operand).  persist: one
-// k_lstm_layer launch (the forward pass), or 33 launches of the per-step k_tc_gemm_p<EPI_LSTM> path, the reference that
-// pb_test_variant_lstm_layer offers for it.  q8 (layer 0, persistent only): the layer writes the int8 slices of h for
-// k_lstm_layer_q8 into T.yenc_lo instead of the fp16 lo tiles.
+// launch (the forward pass), or 33 launches of the per-step k_tc_gemm_p<EPI_LSTM> path, the reference that
+// pb_test_variant_lstm_layer offers for it.  The persistent encoder layer with a hi-only h-part runs k_lstm_layer_enc (h kept
+// in shared memory); k_lstm_layer runs the rest (the decoder of mode 1, and an encoder h-part with all three products,
+// whose hi + lo h would need 128 KB per step buffer).  q8 (layer 0, persistent, hi-only h-part): the layer writes the int8
+// slices of h for k_lstm_layer_q8 into T.yenc_lo instead of the fp16 lo tiles.
 static int variant_lstm_layer_tc(pb_variant_net *N, int layer, int64_t B, bool lo_x, bool lo_h, bool persist, float *y_f32,
                                  cudaStream_t st, bool q8 = false) {
     TcVariant &T = N->tc;
@@ -238,12 +245,14 @@ static int variant_lstm_layer_tc(pb_variant_net *N, int layer, int64_t B, bool l
     for (int d = 0; d < 2; d++)
         if (W[d].nkt_x != x_nkt || W[d].nkt_h != 8) { set_error("unexpected packed LSTM weight shape"); return PB_ERR_STATE; }
     if (persist) {
-        // one launch per layer: every CTA keeps its (direction, row tile) for all 33 steps (k_lstm_layer)
+        // one launch per layer: every CTA keeps its (direction, row tile) for all 33 steps
+        const bool enc = layer == 0 && !lo_h;
         tc::LstmLayer L;
         memset(&L, 0, sizeof(L));
         L.x_hi = x_hi; L.x_lo = x_lo; L.x_mt_stride = x_mt_stride; L.x_nkt = x_nkt;
         for (int d = 0; d < 2; d++) {
             L.w_hi[d] = W[d].w_hi.as<bf16>(); L.w_lo[d] = W[d].w_lo.as<bf16>();
+            L.wh_hi[d] = W[d].wh_hi.as<bf16>(); L.wh_lo[d] = W[d].wh_lo.as<bf16>();
             L.bias[d] = W[d].bias.as<float>();
             L.inv_scale[d] = 1.f / W[d].scale;
             L.c[d] = T.c.as<float>() + (int64_t) d * VH * Bp;
@@ -252,8 +261,9 @@ static int variant_lstm_layer_tc(pb_variant_net *N, int layer, int64_t B, bool l
         if (y_f32) { L.y_f32 = y_f32; L.ldy = (int64_t) VT * 512; }
         L.M = (int) B; L.n_mt = (int) Mt; L.T = VT;
         L.lo_x = lo_x; L.lo_h = lo_h;
+        if (enc && !L.wh_hi[0]) { set_error("encoder weights without their half-tile packing"); return PB_ERR_STATE; }
         if (q8) {
-            if (layer != 0 || lo_h) { set_error("int8 slice output: encoder layer with a hi-only h-part"); return PB_ERR_STATE; }
+            if (!enc) { set_error("int8 slice output: encoder layer with a hi-only h-part"); return PB_ERR_STATE; }
             L.q1 = T.yenc_lo.as<int8_t>(); L.q0 = L.q1 + Mt * q_mt_bytes(); L.q_mt_stride = q_mt_bytes();
         }
 #ifdef PB_LSTM_TRACE
@@ -262,12 +272,14 @@ static int variant_lstm_layer_tc(pb_variant_net *N, int layer, int64_t B, bool l
 #endif
         static bool attr_set = false;
         if (!attr_set) {
-            PB_CUDA(cudaFuncSetAttribute(tc::k_lstm_layer<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::LSTM_SMEM_BYTES));
-            PB_CUDA(cudaFuncSetAttribute(tc::k_lstm_layer<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::LSTM_SMEM_BYTES));
+            PB_CUDA(cudaFuncSetAttribute(tc::k_lstm_layer, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::LSTM_SMEM_BYTES));
+            PB_CUDA(cudaFuncSetAttribute(tc::k_lstm_layer_enc<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::ESMEM_BYTES));
+            PB_CUDA(cudaFuncSetAttribute(tc::k_lstm_layer_enc<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::ESMEM_BYTES));
             attr_set = true;
         }
-        if (q8) tc::k_lstm_layer<true><<<(unsigned) (2 * Mt), tc::LSTM_THREADS, tc::LSTM_SMEM_BYTES, st>>>(L);
-        else tc::k_lstm_layer<false><<<(unsigned) (2 * Mt), tc::LSTM_THREADS, tc::LSTM_SMEM_BYTES, st>>>(L);
+        if (q8) tc::k_lstm_layer_enc<true><<<(unsigned) (2 * Mt), tc::LSTM_THREADS, tc::ESMEM_BYTES, st>>>(L);
+        else if (enc) tc::k_lstm_layer_enc<false><<<(unsigned) (2 * Mt), tc::LSTM_THREADS, tc::ESMEM_BYTES, st>>>(L);
+        else tc::k_lstm_layer<<<(unsigned) (2 * Mt), tc::LSTM_THREADS, tc::LSTM_SMEM_BYTES, st>>>(L);
         N->launches++;
         return PB_OK;
     }
@@ -790,6 +802,27 @@ extern "C" int pb_test_variant_lstm_layer(pb_variant_net_t *net, int layer, int 
         PB_CUDA(cudaMemcpy(h_y_lo, (layer == 0 ? T.yenc_lo : T.ydec_lo).p, (size_t) seq * 2, cudaMemcpyDeviceToHost));
     }
     if (h_c_final) PB_TRY(read_c_final(T, M, h_c_final));
+    return PB_OK;
+}
+
+// The encoder layer of mode 2 (the forward pass's own launch code): h as the decoder's int8 x slices.  h_x: int8 images
+// [M][33][26].  h_q: the slice images as the layer leaves them in T.yenc_lo, int8 [2][Mt][33][8][128][64] (slice 1, then
+// slice 0; tc_gemm.cuh QSeq layout).  poison: that buffer is first filled with 0xff bytes, which padding rows keep.
+extern "C" int pb_test_variant_enc_q8(pb_variant_net_t *net, int M, const int8_t *h_x, int poison, int8_t *h_q) {
+    if (!net || M <= 0 || !h_x || !h_q) { set_error("pb_test_variant_enc_q8: bad argument"); return PB_ERR_ARG; }
+    PB_CUDA(cudaSetDevice(net->device));
+    TcVariant &T = net->tc;
+    const int64_t Mt = ceil_div(M, 128), Bp = Mt * 128;
+    PB_TRY(variant_reserve_tc(T, M, 2));
+    if (poison) PB_TRY(fill_nan(T.yenc_lo));
+    Scratch S;
+    PB_TRY(S.b[0].reserve((size_t) M * VT * 26));
+    PB_CUDA(cudaMemcpy(S.b[0].p, h_x, (size_t) M * VT * 26, cudaMemcpyHostToDevice));
+    tc::k_tc_pack_images<<<(unsigned) ceil_div(Bp * VT * 4, 256), 256, 0>>>(S.b[0].as<int8_t>(), T.img_op.as<bf16>(), M, VT, 26);
+    PB_TRY(variant_lstm_layer_tc(net, 0, M, true, false, true, nullptr, 0, true));
+    PB_CUDA(cudaGetLastError());
+    PB_CUDA(cudaDeviceSynchronize());
+    PB_CUDA(cudaMemcpy(h_q, T.yenc_lo.p, (size_t) (2 * Mt * q_mt_bytes()), cudaMemcpyDeviceToHost));
     return PB_OK;
 }
 

@@ -20,6 +20,7 @@
 #include "common.cuh"
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <type_traits>
 
 namespace pb {
 namespace tc {
@@ -161,6 +162,23 @@ __device__ __forceinline__ void wgmma_256(float (&d)[128], uint64_t adesc, uint6
           "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
         : "l"(adesc), "l"(bdesc), "r"(1));
 }
+// d[64 x 128] += A[64 x 16] B[128 x 16]^T (k_lstm_layer_enc's half gate tiles); each output gets the sums of wgmma_256
+__device__ __forceinline__ void wgmma_128(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32." OP_PTX "." OP_PTX " "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(1));
+}
 
 // ---------------------------------------------------------------- int8-slice operands (mode 2: decoder LSTM layer and linear_1)
 // A value v in [-1, 1] (an LSTM hidden state) is held as the 16-bit fixed-point integer q = rint(v * 32512) split into two
@@ -300,7 +318,9 @@ __device__ __forceinline__ void mma_tile(float (&acc)[128], uint32_t smem_base, 
 // hidden unit (column 4u + gate), so lane pairs (q, q ^ 1) hold gates {0, 1} and {2, 3} of units 2i + q / 2 for both rows:
 // one exchange gives the even lane all four gates of row rA and the odd lane those of row rA + 8.
 // The packed weights carry a power-of-two scale s, undone exactly by the multiply of the fused multiply-add with the bias.
-__device__ __forceinline__ void gates4(const float (&acc)[128], int i, float2 bz, float inv_s, int q, float (&gt)[4]) {
+// The m64n128 fragment (NACC = 64) is the first half of this one: i < 16, columns of its own 128-column tile.
+template <int NACC>
+__device__ __forceinline__ void gates4(const float (&acc)[NACC], int i, float2 bz, float inv_s, int q, float (&gt)[4]) {
     const float a0 = fmaf(acc[4 * i + 0], inv_s, bz.x), a1 = fmaf(acc[4 * i + 1], inv_s, bz.y);
     const float b0 = fmaf(acc[4 * i + 2], inv_s, bz.x), b1 = fmaf(acc[4 * i + 3], inv_s, bz.y);
     const bool odd = q & 1;
@@ -446,8 +466,9 @@ struct LstmLayer {
     int64_t ldy;
     int M, n_mt, T;
     int lo_x, lo_h;                    // 1: the a_lo x w_hi product of the x-part / h-part is executed (0: two products)
-    int8_t *q1, *q0;                   // k_lstm_layer<true>: h_t as int8 slices for the next layer instead of y_lo (QSeq layout)
+    int8_t *q1, *q0;                   // k_lstm_layer_enc: h_t as int8 slices for the next layer instead of y_lo (QSeq layout)
     int64_t q_mt_stride;               // bytes
+    const op_t *wh_hi[2], *wh_lo[2];   // k_lstm_layer_enc, per direction: [8 half tiles][x_nkt + 8][TILE_ELEMS] (128 gate columns)
 #ifdef PB_LSTM_TRACE
     uint64_t *trace;                   // lstm_trace_words(T) stamps per launch, nullptr: none
 #endif
@@ -461,6 +482,9 @@ struct LstmLayer {
 //   [256 T + (cw * T + t) * 2 + k]     k: 0 __threadfence returned, 1 bar_h arrived
 //   [272 T + t * 3 + k]                producer, t >= 1; k: 0 bar_h wait start, 1 wait end, 2 first h-part copy issued
 //   [275 T + k]                        k: 0 %globaltimer, 1 %clock64 at the start; 2, 3 the same when warp 0 ends
+// k_lstm_layer_enc (no bar_h, producer words stay 0): nt = half tile 0-7 with k: 0 start, 1 first bar_full passed, 2 last
+// k-tile issued, 3 end (the previous half's epilogue runs between 1 and 2); the step words are 0 half 7's epilogue done,
+// 1 h published (named barrier passed), both inside half 0 of step t.
 constexpr int LSTM_TRACE_CTAS = 3;
 __host__ __device__ constexpr int64_t lstm_trace_cta_words(int T) { return 275 * (int64_t) T + 4; }
 __host__ __device__ constexpr int64_t lstm_trace_words(int T) { return LSTM_TRACE_CTAS * lstm_trace_cta_words(T); }
@@ -482,9 +506,6 @@ __device__ __forceinline__ uint64_t trace_gtime() {
 #define LSTM_STAMP(off) do {} while (0)
 #endif
 
-// Q8: the layer feeds the int8-slice decoder (mode 2).  The odd-unit lane writes h_t's two int8 slices to q1 / q0 instead of
-// the fp16 lo words, which nothing reads then (the layer's own h-part runs hi only): still 4 B per cell.
-template <bool Q8>
 __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
     extern __shared__ __align__(128) uint8_t smem[];
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem + PSTAGES * PSTAGE_BYTES);
@@ -579,18 +600,14 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
             // units nt * 64 .. + 63 are operand k-tiles 2 nt, 2 nt + 1 of this step.  Lanes q and q ^ 2 hold units 2 i and
             // 2 i + 1 of the same row: the even-unit lane writes the hi words of the pair, the odd-unit lane the lo words.
             const bool odd_u = q >> 1;
-            op_t *yw = ((Q8 || !odd_u) ? G.y_hi : G.y_lo) + y0 + 2 * nt * TILE_ELEMS;
+            op_t *yw = (odd_u ? G.y_lo : G.y_hi) + y0 + 2 * nt * TILE_ELEMS;
             float *yf = G.y_f32 ? G.y_f32 + (int64_t) row * G.ldy + (int64_t) tt * 512 + dir * 256 + nt * (PBN / 4) : nullptr;
-            // Q8: units nt * 64 .. + 63 are slice k-tile 4 dir + nt of this step
-            int8_t *qw = nullptr;
-            if constexpr (Q8) qw = (odd_u ? G.q0 : G.q1) + mt * G.q_mt_stride + (int64_t) (tt * 8 + dir * 4 + nt) * QTILE_BYTES + r128 * 16;
 #pragma unroll
             for (int m = 0; m < PBN / 16; m++) {
                 // cells i = 2 m, 2 m + 1: their two 4 B operand words are adjacent in row r128 and go out as one 8 B store
                 // (lanes 4 apart fill the other half of the 32 B sector); four cells per 16 B store need registers the
                 // 168-register launch does not have (68 B of spills)
                 uint32_t w[2];
-                int uq[4];
 #pragma unroll
                 for (int e = 0; e < 2; e++) {
                     const int i = 2 * m + e;
@@ -601,24 +618,13 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
                     c_prev[i] = cn;
                     const float hp = __shfl_xor_sync(0xffffffffu, hn, 2);
                     const float h0 = odd_u ? hp : hn, h1 = odd_u ? hn : hp;          // units 2 i, 2 i + 1
-                    if constexpr (Q8) {
-                        uq[2 * e] = qbias(h0); uq[2 * e + 1] = qbias(h1);
-                        w[e] = (uint32_t) op_bits_unit(h0) | ((uint32_t) op_bits_unit(h1) << 16);
-                    } else {
-                        uint32_t hi, lo;
-                        split2<true>(h0, h1, hi, lo);
-                        w[e] = odd_u ? lo : hi;
-                    }
+                    uint32_t hi, lo;
+                    split2<true>(h0, h1, hi, lo);
+                    w[e] = odd_u ? lo : hi;
                     if (yf && valid && !odd_u) *reinterpret_cast<float2 *>(yf + 2 * i) = make_float2(h0, h1);
                 }
-                if constexpr (Q8) {
-                    // the even-unit lane writes the hi words and slice 1 of units nt * 64 + 4 m .. + 3, the odd-unit lane slice 0
-                    if (valid && !odd_u) __stwb(reinterpret_cast<uint2 *>(yw + (m >> 3) * TILE_ELEMS + ((m >> 1) & 3) * 1024 + 4 * (m & 1)), make_uint2(w[0], w[1]));
-                    if (valid) __stwb(reinterpret_cast<uint32_t *>(qw + (m >> 2) * 2048 + 4 * (m & 3)), qword(uq[0], uq[1], uq[2], uq[3], odd_u));
-                } else {
-                    // element (unit nt * 64 + 4 m, row r128) of the step's operand tiles, relative to the lane's base
-                    if (valid) __stwb(reinterpret_cast<uint2 *>(yw + (m >> 3) * TILE_ELEMS + ((m >> 1) & 3) * 1024 + 4 * (m & 1)), make_uint2(w[0], w[1]));
-                }
+                // element (unit nt * 64 + 4 m, row r128) of the step's operand tiles, relative to the lane's base
+                if (valid) __stwb(reinterpret_cast<uint2 *>(yw + (m >> 3) * TILE_ELEMS + ((m >> 1) & 3) * 1024 + 4 * (m & 1)), make_uint2(w[0], w[1]));
                 // cells 2 m - 2 .. 2 m + 1 are done: one 16 B store
                 if ((m & 1) && valid) {
                     const int k = m >> 1;
@@ -634,6 +640,265 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer(LstmLayer G) {
         if (lane == 0) mbar_arrive(bar_h);
         LSTM_STAMP(256 * G.T + (warp * G.T + t) * 2 + 1);
     }
+#ifdef PB_LSTM_TRACE
+    if (tr && threadIdx.x == 0) { tr[275 * G.T + 2] = trace_gtime(); tr[275 * G.T + 3] = trace_clock(); }
+#endif
+}
+
+// ---------------------------------------------------------------- persistent encoder LSTM layer, h on chip (variant)
+// k_lstm_layer's grid and arithmetic for the encoder layer with a hi-only h-part (lo_h == 0, x = the int8 images, 1 k-tile).
+// Two changes:
+//  * h stays in shared memory.  A warpgroup's h-part at step t + 1 is exactly the rows its own epilogues wrote at step t, so
+//    each epilogue also writes its hi words into the step's shared h-part (operand tile layout, double-buffered by step
+//    parity), and a per-warpgroup named barrier after a generic -> async proxy fence replaces bar_h, the __threadfence and
+//    the producer's reload of h through L2.  The global h stores are k_lstm_layer's (y_hi and the odd lanes' y_lo words,
+//    y_f32), except that Q8 writes the decoder's int8 slices alone (enc_cells); the next layer and the test hooks read them,
+//    nothing in this kernel does.
+//  * Each step is 8 half gate tiles of 128 columns (32 units x 4 gates, m64n128) into two accumulator sets, and the cell
+//    epilogue of half h runs one unit pair per k-tile between the wgmma groups of half h + 1, so the tensor cores stay busy
+//    while it runs.  Each output element gets the same products in the same order as in k_lstm_layer.
+// The ring carries the 16 KB of weights (hi + lo) of one half-tile k-tile, from the half-tile packing wh_hi / wh_lo; the step's
+// image k-tile has a two-slot buffer of its own, loaded once per step.  Shared memory: 2 x 64 KB h + 2 x 8 KB x + 4 x 16 KB
+// ring + 4 KB bias + barriers = 217,344 B.
+// At a step boundary the x k-tile and the h k-tiles 0-6 of half 0 (written by halves 0-6, published by the barrier after
+// half 6's epilogue) run under half 7's epilogue; only h k-tile 7 waits for it.
+constexpr int EH_BYTES = 8 * TILE_BYTES;                         // one step's h-part: 8 k-tiles of 128 rows
+constexpr int ESTAGES = 4;
+constexpr int ESTAGE_BYTES = 2 * TILE_BYTES;                     // W hi + lo of one half-tile k-tile
+constexpr int ENC_NKT = 9;                                       // k-tiles per half tile from step 1 on: [x | h 0..7]
+constexpr int ESMEM_BYTES = 2 * EH_BYTES + 2 * TILE_BYTES + ESTAGES * ESTAGE_BYTES + 1024 * 4 + 256;
+
+// where the epilogue of one half tile writes: bias, cell states, global h words / slices / fp32 copy, shared h words
+struct EncEpi {
+    const float *sb;
+    float4 *cp;
+    op_t *yw;
+    int8_t *qw;
+    float *yf;
+    uint32_t hs;
+};
+
+// Cells 2 m, 2 m + 1 of the lane's 16 in a half tile: k_lstm_layer's epilogue arithmetic and stores.  Q8: h_t leaves the
+// kernel only as the decoder's two int8 slices (the even-unit lane writes q1, the odd-unit lane q0 of a unit pair): the fp16
+// hi words' one reader was the layer's own h-part, now in shared memory, and the lo words have none (hi-only h-part).
+template <bool Q8>
+__device__ __forceinline__ void enc_cells(const float (&acc)[64], float (&c)[16], int m, const EncEpi &E, float inv_s, int q,
+                                          bool odd_u, bool valid) {
+    uint32_t w[2];
+    int uq[4];
+#pragma unroll
+    for (int e = 0; e < 2; e++) {
+        const int i = 2 * m + e;
+        float gt[4];
+        gates4(acc, i, *reinterpret_cast<const float2 *>(E.sb + 8 * i), inv_s, q, gt);
+        const float cn = sigm(gt[1]) * c[i] + sigm(gt[0]) * tanh_fast(gt[2]);
+        const float hn = sigm(gt[3]) * tanh_fast(cn);
+        c[i] = cn;
+        const float hp = __shfl_xor_sync(0xffffffffu, hn, 2);
+        const float h0 = odd_u ? hp : hn, h1 = odd_u ? hn : hp;          // units 2 i, 2 i + 1
+        if constexpr (Q8) {
+            uq[2 * e] = qbias(h0); uq[2 * e + 1] = qbias(h1);
+            w[e] = (uint32_t) op_bits_unit(h0) | ((uint32_t) op_bits_unit(h1) << 16);
+        } else {
+            uint32_t hi, lo;
+            split2<true>(h0, h1, hi, lo);
+            w[e] = odd_u ? lo : hi;
+        }
+        if (E.yf && valid && !odd_u) *reinterpret_cast<float2 *>(E.yf + 2 * i) = make_float2(h0, h1);
+    }
+    // element (unit 4 m of the half, row r128) of its operand k-tile, relative to the lane's base
+    const int o = ((m >> 1) & 3) * 1024 + 4 * (m & 1);
+    if constexpr (Q8) {
+        if (valid) __stwb(reinterpret_cast<uint32_t *>(E.qw + (m >> 2) * 2048 + 4 * (m & 3)), qword(uq[0], uq[1], uq[2], uq[3], odd_u));
+    } else {
+        if (valid) __stwb(reinterpret_cast<uint2 *>(E.yw + o), make_uint2(w[0], w[1]));
+    }
+    // the next step's h-part: hi words of every row (a padding row's h only meets its own row of the product)
+    if (!odd_u) asm volatile("st.shared.v2.u32 [%0], {%1, %2};" ::"r"(E.hs + 2 * o), "r"(w[0]), "r"(w[1]) : "memory");
+    if ((m & 1) && valid) {
+        const int k = m >> 1;
+        E.cp[k * 256] = make_float4(c[4 * k], c[4 * k + 1], c[4 * k + 2], c[4 * k + 3]);
+    }
+}
+
+// one k-tile of a half tile as one committed wgmma group: a_hi x w_hi + a_hi x w_lo per 16-k slice (mma_ktile<false>)
+__device__ __forceinline__ void enc_ktile(float (&acc)[64], uint32_t a, uint32_t st) {
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < BK / 16; ks++) {
+        const uint64_t a_hi = smem_desc(a + ks * 4096, 2048);
+        wgmma_128(acc, a_hi, smem_desc(st + ks * 4096, 2048));
+        wgmma_128(acc, a_hi, smem_desc(st + TILE_BYTES + ks * 4096, 2048));
+    }
+    wg_commit();
+}
+
+// this warpgroup's h words written so far are visible to its wgmma reads (all 4 warps' generic stores -> async proxy)
+__device__ __forceinline__ void enc_publish_h(int wg) {
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+}
+
+template <bool Q8>
+__global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer_enc(LstmLayer G) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    constexpr int RING = 2 * EH_BYTES + 2 * TILE_BYTES, BIAS = RING + ESTAGES * ESTAGE_BYTES;
+    float *sbias = reinterpret_cast<float *>(smem + BIAS);
+    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + BIAS + 1024 * 4);
+    const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + ESTAGES);
+    const uint32_t bar_xfull = smem_u32(bars + 2 * ESTAGES), bar_xempty = smem_u32(bars + 2 * ESTAGES + 2);
+    const uint32_t hbuf = smem_u32(smem), xbuf = hbuf + 2 * EH_BYTES, ring = hbuf + RING;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int dir = blockIdx.x / G.n_mt, mt = blockIdx.x % G.n_mt;
+
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < ESTAGES; s++) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, CONS_WARPS); }
+        for (int s = 0; s < 2; s++) { mbar_init(bar_xfull + 8 * s, 1); mbar_init(bar_xempty + 8 * s, CONS_WARPS); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    for (int i = threadIdx.x; i < 4 * PBN; i += LSTM_THREADS) sbias[i] = G.bias[dir][i];
+#ifdef PB_LSTM_TRACE
+    const int ts = blockIdx.x == 0 ? 0 : blockIdx.x == gridDim.x / 2 ? 1 : blockIdx.x == gridDim.x - 1 ? 2 : -1;
+    uint64_t *const tr = G.trace && ts >= 0 ? G.trace + ts * lstm_trace_cta_words(G.T) : nullptr;
+    if (tr && threadIdx.x == 0) { tr[275 * G.T] = trace_gtime(); tr[275 * G.T + 1] = trace_clock(); }
+#endif
+    __syncthreads();
+
+    if (warp >= CONS_WARPS) {
+        reg_dealloc<LSTM_PROD_REGS>();
+        if (threadIdx.x == 32 * CONS_WARPS) {
+            uint32_t g = 0;
+            for (int t = 0; t < G.T; t++) {
+                const int tt = dir ? G.T - 1 - t : t;
+                const uint32_t xs = (uint32_t) t & 1u;
+                mbar_wait(bar_xempty + 8 * xs, (((uint32_t) t >> 1) & 1u) ^ 1u);
+                mbar_expect_tx(bar_xfull + 8 * xs, TILE_BYTES);
+                bulk_g2s(xbuf + xs * TILE_BYTES, G.x_hi + (int64_t) mt * G.x_mt_stride + (int64_t) tt * TILE_ELEMS, TILE_BYTES, bar_xfull + 8 * xs);
+                const int nkt = t > 0 ? ENC_NKT : 1;
+                for (int h = 0; h < 8; h++)
+                    for (int kt = 0; kt < nkt; kt++, g++) {
+                        const uint32_t s = g % ESTAGES;
+                        mbar_wait(bar_empty + 8 * s, ((g / ESTAGES) & 1u) ^ 1u);
+                        mbar_expect_tx(bar_full + 8 * s, ESTAGE_BYTES);
+                        const int64_t woff = ((int64_t) h * ENC_NKT + kt) * TILE_ELEMS;
+                        bulk_g2s(ring + s * ESTAGE_BYTES, G.wh_hi[dir] + woff, TILE_BYTES, bar_full + 8 * s);
+                        bulk_g2s(ring + s * ESTAGE_BYTES + TILE_BYTES, G.wh_lo[dir] + woff, TILE_BYTES, bar_full + 8 * s);
+                    }
+            }
+        }
+        return;
+    }
+    reg_alloc<LSTM_CONS_REGS>();
+    const int wg = warp >> 2, q = lane & 3;
+    const int r128 = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * (q & 1);      // row of this lane's cells
+    const int row = mt * BM + r128;
+    const bool valid = row < G.M, odd_u = q >> 1;
+    const float inv_s = G.inv_scale[dir];
+    float4 *const cl = reinterpret_cast<float4 *>(G.c[dir] + c_index(q >> 1, row));   // this lane's first four cells
+    uint32_t g = 0;
+    float acc0[64], acc1[64], c0[16], c1[16];
+
+    // the epilogue targets of half h of step t: units 32 h .. 32 h + 31 are operand k-tile h of the step (slice k-tile
+    // 4 dir + h / 2, chunks 2 (h & 1), + 1)
+    auto epi_of = [&](int t, int h) {
+        const int tt = dir ? G.T - 1 - t : t;
+        EncEpi E;
+        E.sb = sbias + h * (PBN / 2) + 2 * q;
+        E.cp = cl + h * 1024;
+        E.yw = Q8 ? nullptr : (odd_u ? G.y_lo : G.y_hi) + (int64_t) mt * G.y_mt_stride + (int64_t) (tt * 16 + dir * 8 + h) * TILE_ELEMS + r128 * 8;
+        E.qw = Q8 ? (odd_u ? G.q0 : G.q1) + mt * G.q_mt_stride + (int64_t) (tt * 8 + dir * 4 + (h >> 1)) * QTILE_BYTES + (h & 1) * 4096 + r128 * 16
+                  : nullptr;
+        E.yf = G.y_f32 ? G.y_f32 + (int64_t) row * G.ldy + (int64_t) tt * 512 + dir * 256 + h * 32 : nullptr;
+        E.hs = hbuf + ((uint32_t) t & 1u) * EH_BYTES + h * TILE_BYTES + r128 * 16;
+        return E;
+    };
+    auto release = [&](uint32_t gi) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_empty + 8 * (gi % ESTAGES));
+    };
+
+    // Half h of step t into acc; the epilogue of the half before it (step t, h - 1, or step t - 1, 7) from accp / cp_ in
+    // slices under its k-tiles 1-8.  ODD: h is odd (acc1), so the two sets are compile-time arrays in both calls.
+    auto half = [&](auto odd_tag, int t, int h, float(&acc)[64], float(&cn)[16], float(&accp)[64], float(&cp_)[16]) {
+        constexpr bool ODD = decltype(odd_tag)::value;
+        const bool has_prev = ODD || t > 0 || h > 0;
+        const EncEpi E = has_prev ? epi_of(h > 0 ? t : t - 1, h > 0 ? h - 1 : 7) : EncEpi{};
+#ifdef PB_LSTM_TRACE
+        const int tc0 = ((warp * G.T + t) * 8 + h) * 4;
+#endif
+        LSTM_STAMP(tc0);
+        // this half's cell states, in flight during its k-loop
+        {
+            float4 *p = cl + h * 1024;
+#pragma unroll
+            for (int k = 0; k < 4; k++) {
+                const float4 v = valid ? __ldcg(p + k * 256) : make_float4(0.f, 0.f, 0.f, 0.f);
+                cn[4 * k] = v.x; cn[4 * k + 1] = v.y; cn[4 * k + 2] = v.z; cn[4 * k + 3] = v.w;
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < 64; i++) acc[i] = 0.f;
+        const uint32_t xa = xbuf + ((uint32_t) t & 1u) * TILE_BYTES + (uint32_t) wg * 1024;
+        const uint32_t ha = hbuf + ((uint32_t) (t - 1) & 1u) * EH_BYTES + (uint32_t) wg * 1024;
+        // k-tile 0: the step's image k-tile
+        if (!ODD && h == 0) mbar_wait(bar_xfull + 8 * (t & 1), ((uint32_t) t >> 1) & 1u);
+        mbar_wait(bar_full + 8 * (g % ESTAGES), (g / ESTAGES) & 1u);
+        LSTM_STAMP(tc0 + 1);
+        enc_ktile(acc, xa, ring + (g % ESTAGES) * ESTAGE_BYTES);
+        wg_wait<1>();                                       // the previous half's accumulators are complete
+        if (g > 0) release(g - 1);
+        if (!ODD && h == 0 && t > 0) {                      // every group of step t - 1 is complete: its image slot is free
+            __syncwarp();
+            if (lane == 0) mbar_arrive(bar_xempty + 8 * ((t - 1) & 1));
+        }
+        g++;
+        if (t == 0) {
+            // step 0 has no h-part: the previous half's epilogue runs after the image k-tile
+            LSTM_STAMP(tc0 + 2);
+            if (has_prev) {
+#pragma unroll
+                for (int m = 0; m < 8; m++) enc_cells<Q8>(accp, cp_, m, E, inv_s, q, odd_u, valid);
+            }
+            if (ODD && h == 7) enc_publish_h(wg);
+        } else {
+#pragma unroll
+            for (int kt = 1; kt < ENC_NKT; kt++) {
+                if (!ODD && kt == ENC_NKT - 1 && h == 0) {
+                    // h k-tile 7 is the previous half's output: finish its epilogue and publish it first
+                    enc_cells<Q8>(accp, cp_, 7, E, inv_s, q, odd_u, valid);
+                    LSTM_STAMP(256 * G.T + (warp * G.T + t) * 2);
+                    enc_publish_h(wg);
+                    LSTM_STAMP(256 * G.T + (warp * G.T + t) * 2 + 1);
+                }
+                mbar_wait(bar_full + 8 * (g % ESTAGES), (g / ESTAGES) & 1u);
+                enc_ktile(acc, ha + (kt - 1) * TILE_BYTES, ring + (g % ESTAGES) * ESTAGE_BYTES);
+                if (kt == ENC_NKT - 1) LSTM_STAMP(tc0 + 2);
+                if (ODD || kt < ENC_NKT - 1 || h > 0) enc_cells<Q8>(accp, cp_, kt - 1, E, inv_s, q, odd_u, valid);
+                // h k-tiles 0-6 of the next step (halves 0-6) are written
+                if (ODD && kt == ENC_NKT - 1 && h == 7) enc_publish_h(wg);
+                wg_wait<1>();
+                release(g - 1);
+                g++;
+            }
+        }
+        // no wgmma group stays in flight across the loop's back edge: ptxas serializes every wgmma of the kernel when one
+        // does (it cannot follow wg_wait<1> around a loop), and this wait costs one k-tile's tail per half-tile pair
+        if constexpr (ODD) wg_wait<0>();
+        LSTM_STAMP(tc0 + 3);
+    };
+
+    for (int t = 0; t < G.T; t++) {
+        for (int h = 0; h < 8; h += 2) {
+            half(std::false_type{}, t, h, acc0, c0, acc1, c1);
+            half(std::true_type{}, t, h + 1, acc1, c1, acc0, c0);
+        }
+    }
+    // the last half tile's epilogue
+    wg_wait<0>();
+    release(g - 1);
+    const EncEpi E = epi_of(G.T - 1, 7);
+#pragma unroll
+    for (int m = 0; m < 8; m++) enc_cells<Q8>(acc1, c1, m, E, inv_s, q, odd_u, valid);
 #ifdef PB_LSTM_TRACE
     if (tr && threadIdx.x == 0) { tr[275 * G.T + 2] = trace_gtime(); tr[275 * G.T + 3] = trace_clock(); }
 #endif

@@ -1,13 +1,13 @@
 """Where the time of the LSTM layer kernels goes: per-phase %clock64 stamps of a PB_LSTM_TRACE build (tc_gemm.cuh), for
-both variant LSTM layers of one VariantNet.predict chunk at each size (the encoder's k_lstm_layer and the decoder's
-k_lstm_layer_q8, or k_lstm_layer in mode 1).
+both variant LSTM layers of one VariantNet.predict chunk at each size (the encoder's k_lstm_layer_enc, or k_lstm_layer when
+its h-part runs all three products, and the decoder's k_lstm_layer_q8, or k_lstm_layer in mode 1).
 
     python scripts/trace_lstm_layer.py [--sizes 8448 1408] [--lib TRACED.so] [--build-dir DIR] [--out FILE]
 
 Without --lib the traced library is built with `make EXTRA=-DPB_LSTM_TRACE` into --build-dir (default: a new temporary
 directory), never into the tree.  CTAs 0, n/2 and n-1 are sampled; every phase is the median (and mean) over those CTAs,
-their 8 consumer warps, steps 1..32 and the gate tiles, 4 in k_lstm_layer and 8 in k_lstm_layer_q8 (producer phases: over
-CTAs and steps).  Times are SM cycles; the
+their 8 consumer warps, steps 1..32 and the gate tiles, 4 in k_lstm_layer and 8 in k_lstm_layer_q8, or the 8 half gate tiles
+of k_lstm_layer_enc (producer phases: over CTAs and steps).  Times are SM cycles; the
 kernel's own clock (cycles over %globaltimer) is printed beside the card name, power limit and nvidia-smi's SM clock.
 """
 import argparse
@@ -65,6 +65,18 @@ def phases(words: np.ndarray) -> dict:
         step = w[256 * T:272 * T].reshape(8, T, 2)         # [warp][t][fence returned, bar_h arrived]
         prod = w[272 * T:275 * T].reshape(T, 3)            # [t][bar_h wait start, wait end, first h copy issued]
         tl = tile[:, 1:]
+        if not prod.any():
+            # k_lstm_layer_enc (no bar_h): per half tile [start, first full, last k-tile issued, end], the previous half's
+            # epilogue running between the k-tiles; per step [half 7's epilogue done, h published (named barrier passed)]
+            add("half: start -> first bar_full", tl[..., 1] - tl[..., 0])
+            add("half: first bar_full -> last k-tile issued (previous half's epilogue under it)", tl[..., 2] - tl[..., 1])
+            add("half, even: last k-tile issued -> end", tl[:, :, 0::2, 3] - tl[:, :, 0::2, 2])
+            add("half, odd: last k-tile issued -> end (wg_wait<0>)", tl[:, :, 1::2, 3] - tl[:, :, 1::2, 2])
+            add("half period (start -> next start, same step)", tl[:, :, 1:, 0] - tl[:, :, :-1, 0])
+            add("step: half 7 epilogue done -> h published", step[:, 1:, 1] - step[:, 1:, 0])
+            add("step period (half 0 start -> next half 0 start)", tile[:, 2:, 0, 0] - tile[:, 1:-1, 0, 0])
+            add("kernel (globaltimer, ns)", [meta[2] - meta[0]])
+            continue
         add("tile: start -> first bar_full", tl[..., 1] - tl[..., 0])
         add("tile: first bar_full -> wg_wait<0>", tl[..., 2] - tl[..., 1])
         add("tile: wg_wait<0> -> epilogue end", tl[..., 3] - tl[..., 2])
@@ -135,11 +147,12 @@ def main():
         print(f"\n{sz['candidates']} candidates, {sz['ctas']} CTAs; kernel SM clock: encoder "
               f"{sz['encoder']['kernel_sm_mhz']:.0f} MHz, decoder {sz['decoder']['kernel_sm_mhz']:.0f} MHz")
         print(f"{'phase (SM cycles; median / mean)':<56}{'encoder':>20}{'decoder':>20}")
-        for k in sz["encoder"]:
+        for k in dict.fromkeys(list(sz["encoder"]) + list(sz["decoder"])):
             if k == "kernel_sm_mhz":
                 continue
-            e, d = sz["encoder"][k], sz["decoder"][k]
-            print(f"{k:<56}{e['median']:>11.0f} /{e['mean']:>7.0f}{d['median']:>11.0f} /{d['mean']:>7.0f}")
+            cols = "".join(f"{L[k]['median']:>11.0f} /{L[k]['mean']:>7.0f}" if k in L else f"{'-':>20}"
+                           for L in (sz["encoder"], sz["decoder"]))
+            print(f"{k:<56}{cols}")
     if args.out:
         with open(args.out, "w") as f:
             json.dump(res, f, indent=1)
