@@ -470,9 +470,11 @@ int pb_test_variant_lstm_layer(pb_variant_net_t *net, int layer, int M, const vo
  * slice 0).  poison: that buffer is filled with 0xff bytes first, which padding rows keep. */
 int pb_test_variant_enc_q8(pb_variant_net_t *net, int M, const int8_t *h_x, int poison, int8_t *h_q);
 /* diagnostics: the int8-slice decoder LSTM layer of mode 2 (k_lstm_layer_q8).  h_x: fp32 [M][33][512], quantized on the host
- * to the slices the encoder would write.  persist 0 = one launch per step.  Outputs (each may be NULL): y_f32 [M][33][512];
- * h_q: the layer's own h slices, 2 x ceil(M / 128) x 33 x 8 x 8192 bytes (slice 1, then slice 0; tc_gemm.cuh QSeq layout);
- * c_final [2][256][M].  poison: every buffer the launch touches starts as 0xff bytes. */
+ * to the slices the encoder would write.  persist: 1 = one launch of all 33 steps (the forward pass), 0 = one launch per
+ * step, k >= 2 = launches of k steps (the last one shorter); every split computes the same bits.  Outputs (each may be
+ * NULL): y_f32 [M][33][512]; h_q: the layer's own h slices, 2 x ceil(M / 128) x 33 x 8 x 8192 bytes (slice 1, then slice 0;
+ * tc_gemm.cuh QSeq layout); c_final [2][256][M].  poison: every buffer the launch touches starts as 0xff bytes, y_f32 with
+ * room for the padding rows, and a padding row of y_f32 that does not keep them fails the call with PB_ERR_STATE. */
 int pb_test_variant_lstm_q8(pb_variant_net_t *net, int M, const float *h_x, int persist, int poison, float *h_y_f32, int8_t *h_q,
                             float *h_c_final);
 /* diagnostics: linear_1 of mode 2 (k_gemm_q8, the forward pass's own launch code) with the network's packed weights.  h_q: the

@@ -312,9 +312,10 @@ static int variant_lstm_layer_tc(pb_variant_net *N, int layer, int64_t B, bool l
 }
 
 // The int8-slice decoder layer (mode 2): x = the encoder's slices in T.yenc_lo, h slices in T.ydec_q (its own h-part and
-// linear_1's A operand) (+ the optional fp32 copy).  persist: one k_lstm_layer_q8 launch for all 33
-// steps (the forward pass), or one launch per step, the reference for the in-kernel h hand-off (pb_test_variant_lstm_q8).
-static int variant_dec_q8(pb_variant_net *N, int64_t B, bool persist, float *y_f32, cudaStream_t st) {
+// linear_1's A operand) (+ the optional fp32 copy).  steps: time steps per k_lstm_layer_q8 launch, VT for the forward pass;
+// fewer cut the layer into launches that hand h and c over through HBM, the reference for the in-kernel hand-off
+// (pb_test_variant_lstm_q8).
+static int variant_dec_q8(pb_variant_net *N, int64_t B, int steps, float *y_f32, cudaStream_t st) {
     TcVariant &T = N->tc;
     const int64_t Mt = ceil_div(B, 128), Bp = Mt * 128;
     PB_CUDA(cudaMemsetAsync(T.c.p, 0, sizeof(float) * 2 * VH * Bp, st));
@@ -341,8 +342,8 @@ static int variant_dec_q8(pb_variant_net *N, int64_t B, bool persist, float *y_f
         attr_set = true;
     }
     for (int t0 = 0; t0 < VT; t0 = L.t1) {
-        L.t0 = t0; L.t1 = persist ? VT : t0 + 1;
-        tc::k_lstm_layer_q8<<<(unsigned) (2 * Mt), tc::LSTM_THREADS, tc::QSMEM_BYTES, st>>>(L);
+        L.t0 = t0; L.t1 = std::min(t0 + steps, VT);
+        tc::k_lstm_layer_q8<<<(unsigned) (2 * Mt), tc::LQ_THREADS, tc::QSMEM_BYTES, st>>>(L);
         N->launches++;
     }
     return PB_OK;
@@ -448,7 +449,7 @@ int variant_forward_tc(pb_variant_net *N, const int8_t *d_images, int64_t B, flo
         // int8-slice decoder: the encoder runs its h-part hi only and hands the decoder its h as slices; lo_mask bits 0-2 do not
         // apply (set_lo_mask returns the network to mode 1)
         PB_TRY(variant_lstm_layer_tc(N, 0, B, true, false, true, nullptr, st, true));
-        PB_TRY(variant_dec_q8(N, B, true, d_hidden_dbg, st));
+        PB_TRY(variant_dec_q8(N, B, VT, d_hidden_dbg, st));
     } else {
         PB_TRY(variant_lstm_layer_tc(N, 0, B, true, T.lo_mask & 1, true, nullptr, st));
         PB_TRY(variant_lstm_layer_tc(N, 1, B, (T.lo_mask >> 1) & 1, (T.lo_mask >> 2) & 1, true, d_hidden_dbg, st));
@@ -826,10 +827,11 @@ extern "C" int pb_test_variant_enc_q8(pb_variant_net_t *net, int M, const int8_t
     return PB_OK;
 }
 
-// The int8-slice decoder layer (variant_dec_q8, the forward pass's own launch code) on host-quantized input slices.
+// The int8-slice decoder layer (variant_dec_q8, the forward pass's own launch code) on host-quantized input slices.  persist:
+// 1 one launch, 0 one launch per step, k >= 2 launches of k steps.
 extern "C" int pb_test_variant_lstm_q8(pb_variant_net_t *net, int M, const float *h_x, int persist, int poison, float *h_y_f32, int8_t *h_q,
                                        float *h_c_final) {
-    if (!net || M <= 0 || !h_x) { set_error("pb_test_variant_lstm_q8: bad argument"); return PB_ERR_ARG; }
+    if (!net || M <= 0 || !h_x || persist < 0) { set_error("pb_test_variant_lstm_q8: bad argument"); return PB_ERR_ARG; }
     PB_CUDA(cudaSetDevice(net->device));
     TcVariant &T = net->tc;
     const int64_t Mt = ceil_div(M, 128), qbytes = Mt * q_mt_bytes();
@@ -848,14 +850,26 @@ extern "C" int pb_test_variant_lstm_q8(pb_variant_net_t *net, int M, const float
         }
     PB_CUDA(cudaMemcpy(T.yenc_lo.p, q.data(), q.size(), cudaMemcpyHostToDevice));
     Scratch S;
+    // y_f32 with room for the padding rows too: under poison they must come back as the 0xff bytes they started as
+    const size_t y_rows = (size_t) (poison ? Mt * 128 : M), y_row_bytes = sizeof(float) * VT * 512;
     if (h_y_f32) {
-        PB_TRY(S.b[0].reserve(sizeof(float) * (size_t) M * VT * 512));
+        PB_TRY(S.b[0].reserve(y_rows * y_row_bytes));
         PB_CUDA(cudaMemset(S.b[0].p, poison ? 0xff : 0, S.b[0].cap));
     }
-    PB_TRY(variant_dec_q8(net, M, persist != 0, h_y_f32 ? S.b[0].as<float>() : nullptr, 0));
+    PB_TRY(variant_dec_q8(net, M, persist == 0 ? 1 : persist == 1 ? VT : persist, h_y_f32 ? S.b[0].as<float>() : nullptr, 0));
     PB_CUDA(cudaGetLastError());
     PB_CUDA(cudaDeviceSynchronize());
-    if (h_y_f32) PB_CUDA(cudaMemcpy(h_y_f32, S.b[0].p, sizeof(float) * (size_t) M * VT * 512, cudaMemcpyDeviceToHost));
+    if (h_y_f32) {
+        PB_CUDA(cudaMemcpy(h_y_f32, S.b[0].p, (size_t) M * y_row_bytes, cudaMemcpyDeviceToHost));
+        if (y_rows > (size_t) M) {
+            std::vector<uint8_t> pad((y_rows - M) * y_row_bytes);
+            PB_CUDA(cudaMemcpy(pad.data(), S.b[0].as<uint8_t>() + (size_t) M * y_row_bytes, pad.size(), cudaMemcpyDeviceToHost));
+            if (std::any_of(pad.begin(), pad.end(), [](uint8_t v) { return v != 0xff; })) {
+                set_error("pb_test_variant_lstm_q8: a padding row of y_f32 was written");
+                return PB_ERR_STATE;
+            }
+        }
+    }
     if (h_q) PB_CUDA(cudaMemcpy(h_q, T.ydec_q.p, (size_t) (2 * qbytes), cudaMemcpyDeviceToHost));
     if (h_c_final) PB_TRY(read_c_final(T, M, h_c_final));
     return PB_OK;

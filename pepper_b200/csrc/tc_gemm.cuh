@@ -194,10 +194,19 @@ __device__ __forceinline__ void wgmma_128(float (&d)[64], uint64_t adesc, uint64
 constexpr int QK = 64;                              // k per ring stage
 constexpr int QTILE_BYTES = 128 * QK;               // 8 KB: one slice of a 128 x 64 tile
 constexpr int QN = 128;                             // gate columns per tile (32 hidden units x 4 gates)
-constexpr int QSTAGES = 6;
+constexpr int QSTAGES = 6;                          // k_gemm_q8's ring
 constexpr int QSTAGE_BYTES = 4 * QTILE_BYTES;       // a1, a0, w1, w0 = 32 KB
-constexpr int QSMEM_BYTES = QSTAGES * QSTAGE_BYTES + 256 + 2 * 1024 * 4;   // ring + barriers + bias + column scales
 constexpr int GQSMEM_BYTES = QSTAGES * QSTAGE_BYTES + 256;                  // k_gemm_q8: ring + barriers
+// k_lstm_layer_q8: a 4-stage ring, one gate tile's fp32 pre-activations (128 rows x 128 columns) staged for the epilogue
+// warpgroup, barriers, bias and column scales = 205,056 B
+constexpr int LQSTAGES = 4;
+constexpr int QPRE_BYTES = BM * QN * 4;
+constexpr int QSMEM_BYTES = LQSTAGES * QSTAGE_BYTES + QPRE_BYTES + 256 + 2 * 1024 * 4;
+// warps 0-7 consumers, 8-11 the epilogue warpgroup, 12-15 the producer warpgroup (one issuing thread); the setmaxnreg split
+// 24 + 2 x 168 + 152 = 4 x 128 is the launch's register file
+constexpr int LQ_THREADS = 512;
+constexpr int LQ_EPI_WARP = 8, LQ_PROD_WARP = 12;
+constexpr int LQ_PROD_REGS = 24, LQ_CONS_REGS = 168, LQ_EPI_REGS = 152;
 constexpr float QSCALE = 32512.f;
 
 // d[64 x 128] (s32) += A[64 x 32] B[128 x 32]^T, s8 operands K-major in shared memory
@@ -482,11 +491,16 @@ struct LstmLayer {
 //   [256 T + (cw * T + t) * 2 + k]     k: 0 __threadfence returned, 1 bar_h arrived
 //   [272 T + t * 3 + k]                producer, t >= 1; k: 0 bar_h wait start, 1 wait end, 2 first h-part copy issued
 //   [275 T + k]                        k: 0 %globaltimer, 1 %clock64 at the start; 2, 3 the same when warp 0 ends
+//   [275 T + 4 + ((ew * T + t) * 8 + nt) * 4 + k]   k_lstm_layer_q8's epilogue warps ew = 0-3; k: 0 "staged" wait issued,
+//                                      1 cells done (slices and c stored), 2 h_t published (bar_h arrived; nt = 7 only).
+//                                      bar.sync defers its blocking to the next memory access, so a clock read right after
+//                                      it would not mark the release: the consumers' "staging stored" stamps bound it.
 // k_lstm_layer_enc (no bar_h, producer words stay 0): nt = half tile 0-7 with k: 0 start, 1 first bar_full passed, 2 last
 // k-tile issued, 3 end (the previous half's epilogue runs between 1 and 2); the step words are 0 half 7's epilogue done,
-// 1 h published (named barrier passed), both inside half 0 of step t.
+// 1 h published (named barrier passed), both inside half 0 of step t.  In k_lstm_layer_q8 the consumers' k = 3 is
+// "staging stored" and their step words stay 0 (the epilogue warps publish h).
 constexpr int LSTM_TRACE_CTAS = 3;
-__host__ __device__ constexpr int64_t lstm_trace_cta_words(int T) { return 275 * (int64_t) T + 4; }
+__host__ __device__ constexpr int64_t lstm_trace_cta_words(int T) { return 403 * (int64_t) T + 4; }
 __host__ __device__ constexpr int64_t lstm_trace_words(int T) { return LSTM_TRACE_CTAS * lstm_trace_cta_words(T); }
 __device__ __forceinline__ uint64_t trace_clock() {
     uint64_t c;
@@ -910,7 +924,36 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer_enc(LstmLayer G)
 // 64, 128-column gate tiles (32 units x 4 gates, 8 per step) so that the two int32 accumulators of a warpgroup take the 128
 // registers one fp32 accumulator took.  Each step writes h_t only as int8 slices: they are the h-part of its own next step and,
 // all 33 steps together, the A operand of linear_1 (k_gemm_q8).  Steps t0 .. t1 - 1 run in one launch: the cell state and h
-// stay in HBM between launches, so one launch per step is the cross-check of the in-kernel hand-off.
+// stay in HBM between launches, so launches of fewer steps are the cross-check of the in-kernel hand-off.
+//
+// The cell epilogue runs in a warpgroup of its own, under the next gate tile's k-loop.  The consumers' two accumulators leave
+// no registers for a second set, so the hand-off goes through shared memory: once a tile's k-loop ends, the consumers fold
+// hh / mix into fp32 pre-activations, fmaf(fmaf(hh, 256, mix), scale, bias), store them to the 64 KB staging buffer and go on
+// to the next tile; epilogue thread r (0-127) runs the 32 cells of row r from there, writes the q1 / q0 slices (two 16 B
+// chunks each), c and the optional y_f32, and after gate tile 7 publishes h_t to the producer.  Padding rows write nothing.
+//
+// Staging buffer: the pre-activation of (row r, unit j of the tile, gate g) sits at byte
+//   j * 2048 + (r / 8) * 128 + ((r % 8) ^ 4 (j & 1)) * 16 + 4 g
+// An epilogue thread reads a cell's four gates with one 16 B load, 8 consecutive rows of one unit filling one 128 B line.  A
+// consumer lane stores two gates (8 B) of one unit and row; the XOR by unit parity puts the two units of a half-warp's
+// store on disjoint banks, so each warp-wide store takes 2 wavefronts, the minimum for 256 B.
+//
+// Barriers (g: the launch's running k-tile count; n = 0 .. N - 1: its gate tiles, N = 8 (t1 - t0)):
+//   bar_full[s]   mbarrier, count 1: the producer's arrive.expect_tx, completed by the bulk copies' bytes.  Every consumer
+//                 warp waits on stage g % LQSTAGES with parity (g / LQSTAGES) & 1.
+//   bar_empty[s]  mbarrier, count 8: lane 0 of each consumer warp, once the wgmma group that read the stage is complete.
+//                 The producer waits before it refills the stage for k-tile g, with parity ((g / LQSTAGES) & 1) ^ 1.
+//   bar_h         mbarrier, count 4: lane 0 of each epilogue warp after gate tile 7 of step t, its h_t slices written and
+//                 __threadfence'd; that completes phase t - t0.  The producer waits on it with parity (t - t0) & 1, then
+//                 fence.proxy.async, before the first h-part copy of step t + 1.  The launch's last phase has no waiter.
+//   STAGED        named barrier 1, 384 threads: the 256 consumers bar.arrive once tile n is in the staging buffer; the 128
+//                 epilogue threads bar.sync before reading it.  N times.
+//   FREE          named barrier 2, 384 threads: the epilogue threads bar.arrive once they have read tile n, n < N - 1; the
+//                 consumers bar.sync before storing tile n + 1.  N - 1 times, so no barrier is left half-arrived at exit.
+// Each waits for the other before its next arrival, so neither named barrier ever has two generations in flight.  Every
+// count and parity starts from the launch's first step, so a launch at t0 > 0 starts like the first one; c and the h
+// slices of step t0 - 1 come from HBM, written by the previous launch.  The kernel ends when the epilogue warps have
+// written the last tile.
 struct LstmLayerQ {
     const int8_t *x1, *x0;             // input sequence slices (QSeq): tile (mt, tt, kt) at mt * q_mt_stride + (tt * 8 + kt) * QTILE_BYTES
     const int8_t *w1[2], *w0[2];       // per direction: [8 n-tiles][12 k-tiles][QTILE_BYTES]
@@ -927,9 +970,10 @@ struct LstmLayerQ {
 #endif
 };
 
+template <int NS>
 __device__ __forceinline__ void load_stage_q(uint32_t smem_base, uint32_t bar_full, uint32_t bar_empty, uint32_t g, const int8_t *a1,
                                              const int8_t *a0, const int8_t *w1, const int8_t *w0) {
-    const uint32_t s = g % QSTAGES, ph = (g / QSTAGES) & 1u;
+    const uint32_t s = g % NS, ph = (g / NS) & 1u;
     mbar_wait(bar_empty + 8 * s, ph ^ 1u);
     const uint32_t st = smem_base + s * QSTAGE_BYTES;
     mbar_expect_tx(bar_full + 8 * s, QSTAGE_BYTES);
@@ -939,23 +983,29 @@ __device__ __forceinline__ void load_stage_q(uint32_t smem_base, uint32_t bar_fu
     bulk_g2s(st + 3 * QTILE_BYTES, w0, QTILE_BYTES, bar_full + 8 * s);
 }
 
-__global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer_q8(LstmLayerQ G) {
+__device__ __forceinline__ void named_arrive(int id, int threads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+__device__ __forceinline__ void named_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+constexpr int LQ_STAGED = 1, LQ_FREE = 2, LQ_HANDOFF_THREADS = 32 * LQ_PROD_WARP;   // named barriers of warps 0-11
+
+__global__ void __launch_bounds__(LQ_THREADS, 1) k_lstm_layer_q8(LstmLayerQ G) {
     extern __shared__ __align__(128) uint8_t smem[];
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + QSTAGES * QSTAGE_BYTES);
-    float *sbias = reinterpret_cast<float *>(smem + QSTAGES * QSTAGE_BYTES + 256);
+    constexpr int PRE = LQSTAGES * QSTAGE_BYTES, BARS = PRE + QPRE_BYTES;
+    constexpr int X_NKT = 8, W_NKT = 12, N_TILES = 8;
+    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + BARS);
+    float *sbias = reinterpret_cast<float *>(smem + BARS + 256);
     float *sscale = sbias + 1024;
-    const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + QSTAGES), bar_h = smem_u32(bars + 2 * QSTAGES);
+    const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + LQSTAGES), bar_h = smem_u32(bars + 2 * LQSTAGES);
     const uint32_t smem_base = smem_u32(smem);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int dir = blockIdx.x / G.n_mt, mt = blockIdx.x % G.n_mt;
-    constexpr int X_NKT = 8, W_NKT = 12, N_TILES = 8;
+    const int n_tiles = (G.t1 - G.t0) * N_TILES;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < QSTAGES; s++) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, CONS_WARPS); }
-        mbar_init(bar_h, CONS_WARPS);
+        for (int s = 0; s < LQSTAGES; s++) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, CONS_WARPS); }
+        mbar_init(bar_h, LQ_PROD_WARP - LQ_EPI_WARP);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    for (int i = threadIdx.x; i < 1024; i += LSTM_THREADS) { sbias[i] = G.bias[dir][i]; sscale[i] = G.col_scale[dir][i]; }
+    for (int i = threadIdx.x; i < 1024; i += LQ_THREADS) { sbias[i] = G.bias[dir][i]; sscale[i] = G.col_scale[dir][i]; }
 #ifdef PB_LSTM_TRACE
     const int ts = blockIdx.x == 0 ? 0 : blockIdx.x == gridDim.x / 2 ? 1 : blockIdx.x == gridDim.x - 1 ? 2 : -1;
     uint64_t *const tr = G.trace && ts >= 0 ? G.trace + ts * lstm_trace_cta_words(G.T) : nullptr;
@@ -963,9 +1013,9 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer_q8(LstmLayerQ G)
 #endif
     __syncthreads();
 
-    if (warp >= CONS_WARPS) {
-        reg_dealloc<LSTM_PROD_REGS>();
-        if (threadIdx.x == 32 * CONS_WARPS) {
+    if (warp >= LQ_PROD_WARP) {
+        reg_dealloc<LQ_PROD_REGS>();
+        if (threadIdx.x == 32 * LQ_PROD_WARP) {
             uint32_t g = 0;
             for (int t = G.t0; t < G.t1; t++) {
                 const int tt = dir ? G.T - 1 - t : t, tp = dir ? tt + 1 : tt - 1;
@@ -978,7 +1028,7 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer_q8(LstmLayerQ G)
                             a1 = G.x1 + off; a0 = G.x0 + off;
                         } else {
                             if (kt == X_NKT && nt == 0 && t > G.t0) {
-                                // every consumer warp has written its part of h_{t-1}: make it visible to the bulk-copy engine
+                                // every epilogue warp has written its rows of h_{t-1}: make them visible to the bulk-copy engine
                                 LSTM_STAMP(272 * G.T + t * 3);
                                 mbar_wait(bar_h, (uint32_t) (t - G.t0 - 1) & 1u);
                                 asm volatile("fence.proxy.async;" ::: "memory");
@@ -988,7 +1038,7 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer_q8(LstmLayerQ G)
                             a1 = G.q1 + off; a0 = G.q0 + off;
                         }
                         const int64_t woff = ((int64_t) nt * W_NKT + kt) * QTILE_BYTES;
-                        load_stage_q(smem_base, bar_full, bar_empty, g, a1, a0, G.w1[dir] + woff, G.w0[dir] + woff);
+                        load_stage_q<LQSTAGES>(smem_base, bar_full, bar_empty, g, a1, a0, G.w1[dir] + woff, G.w0[dir] + woff);
                         if (t > G.t0 && nt == 0 && kt == X_NKT) LSTM_STAMP(272 * G.T + t * 3 + 2);
                     }
                 }
@@ -996,35 +1046,103 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer_q8(LstmLayerQ G)
         }
         return;
     }
-    reg_alloc<LSTM_CONS_REGS>();
+
+    if (warp >= LQ_EPI_WARP) {
+        reg_alloc<LQ_EPI_REGS>();
+        const int r128 = threadIdx.x - 32 * LQ_EPI_WARP;                // the row of this thread's cells
+        const int row = mt * BM + r128;
+        const bool valid = row < G.M;
+        // cells (nt * 32 + 8 a + b + 2 k, row) of c_index sit at cl[(nt * 4 + a) * 256 + 2 b], element k
+        float4 *const cl = reinterpret_cast<float4 *>(G.c[dir] + c_index(0, row));
+        const uint8_t *const srow = smem + PRE + (r128 >> 3) * 128;
+        const int rx = r128 & 7;
+        int n = 0;
+        for (int t = G.t0; t < G.t1; t++) {
+            const int tt = dir ? G.T - 1 - t : t;
+            const int64_t qo = (int64_t) mt * G.q_mt_stride + (int64_t) (tt * 8 + dir * 4) * QTILE_BYTES + r128 * 16;
+            float *yf = G.y_f32 ? G.y_f32 + (int64_t) row * G.ldy + (int64_t) tt * 512 + dir * 256 : nullptr;
+            for (int nt = 0; nt < N_TILES; nt++, n++) {
+#ifdef PB_LSTM_TRACE
+                const int te0 = 275 * G.T + 4 + (((warp - LQ_EPI_WARP) * G.T + t) * 8 + nt) * 4;
+#endif
+                // the tile's 32 cell states, in flight while the consumers fold and stage
+                float4 *cp = cl + nt * 4 * 256;
+                float c[QN / 4];
+#pragma unroll
+                for (int a = 0; a < 4; a++)
+#pragma unroll
+                    for (int b = 0; b < 2; b++) {
+                        const float4 v = valid ? __ldcg(cp + a * 256 + 2 * b) : make_float4(0.f, 0.f, 0.f, 0.f);
+                        c[8 * a + b] = v.x; c[8 * a + b + 2] = v.y; c[8 * a + b + 4] = v.z; c[8 * a + b + 6] = v.w;
+                    }
+                LSTM_STAMP(te0);
+                named_sync(LQ_STAGED, LQ_HANDOFF_THREADS);
+                uint32_t w1[8], w0[8];
+#pragma unroll
+                for (int m = 0; m < 8; m++) {
+                    // units 4 m .. 4 m + 3 of the tile: four independent cells, one word of each slice
+                    int uq[4];
+                    float h[4];
+#pragma unroll
+                    for (int e = 0; e < 4; e++) {
+                        const int j = 4 * m + e;
+                        const float4 gt = *reinterpret_cast<const float4 *>(srow + j * 2048 + ((rx ^ ((j & 1) << 2)) << 4));
+                        const float cn = sigm(gt.y) * c[j] + sigm(gt.x) * tanh_fast(gt.z);
+                        h[e] = sigm(gt.w) * tanh_fast(cn);
+                        c[j] = cn;
+                        uq[e] = qbias(h[e]);
+                    }
+                    w1[m] = qword(uq[0], uq[1], uq[2], uq[3], false);
+                    w0[m] = qword(uq[0], uq[1], uq[2], uq[3], true);
+                    if (yf && valid) *reinterpret_cast<float4 *>(yf + nt * (QN / 4) + 4 * m) = make_float4(h[0], h[1], h[2], h[3]);
+                }
+                if (n + 1 < n_tiles) named_arrive(LQ_FREE, LQ_HANDOFF_THREADS);
+                if (valid) {
+                    // units nt * 32 .. + 31 are chunks 2 (nt & 1), + 1 of slice k-tile 4 dir + nt / 2
+                    const int64_t o = qo + (nt >> 1) * QTILE_BYTES + (nt & 1) * 2 * 2048;
+                    __stwb(reinterpret_cast<uint4 *>(G.q1 + o), make_uint4(w1[0], w1[1], w1[2], w1[3]));
+                    __stwb(reinterpret_cast<uint4 *>(G.q1 + o + 2048), make_uint4(w1[4], w1[5], w1[6], w1[7]));
+                    __stwb(reinterpret_cast<uint4 *>(G.q0 + o), make_uint4(w0[0], w0[1], w0[2], w0[3]));
+                    __stwb(reinterpret_cast<uint4 *>(G.q0 + o + 2048), make_uint4(w0[4], w0[5], w0[6], w0[7]));
+#pragma unroll
+                    for (int a = 0; a < 4; a++)
+#pragma unroll
+                        for (int b = 0; b < 2; b++)
+                            cp[a * 256 + 2 * b] = make_float4(c[8 * a + b], c[8 * a + b + 2], c[8 * a + b + 4], c[8 * a + b + 6]);
+                }
+                LSTM_STAMP(te0 + 1);
+            }
+            // h_t of this warp's rows is complete (all eight gate tiles): publish it to the producer thread
+            __threadfence();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(bar_h);
+            LSTM_STAMP(275 * G.T + 4 + (((warp - LQ_EPI_WARP) * G.T + t) * 8 + 7) * 4 + 2);
+        }
+        return;
+    }
+
+    reg_alloc<LQ_CONS_REGS>();
     const int wg = warp >> 2, q = lane & 3;
-    const int r128 = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * (q & 1);      // row of this lane's cells
-    const int row = mt * BM + r128;
-    const bool valid = row < G.M;
-    const bool odd_u = q >> 1;
-    float4 *const cl = reinterpret_cast<float4 *>(G.c[dir] + c_index(q >> 1, row));   // this lane's first four cells
+    const int rA = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    // accumulator fragment of m64n128: [4 i + 2 h + e] is row rA + 8 h, column 8 i + 2 q + e = gate 2 (q & 1) + e of unit
+    // 2 i + q / 2.  This lane's staging slot of (unit q / 2, row rA); unit 2 i + q / 2 and row rA + 8 h are i * 4096 + h * 128
+    // bytes on (2 i is even, so the unit parity, and with it the XOR, is the lane's own).
+    float *const sp = reinterpret_cast<float *>(smem + PRE + (q >> 1) * 2048 + (rA >> 3) * 128 + ((((lane >> 2) ^ ((q >> 1) << 2))) << 4) +
+                                                (q & 1) * 8);
     uint32_t g = 0;
+    int n = 0;
     int hh[64], mix[64];
     for (int t = G.t0; t < G.t1; t++) {
-        const int tt = dir ? G.T - 1 - t : t;
         const int nkt = X_NKT + (t > 0 ? W_NKT - X_NKT : 0);
-        for (int nt = 0; nt < N_TILES; nt++) {
+        for (int nt = 0; nt < N_TILES; nt++, n++) {
 #ifdef PB_LSTM_TRACE
             const int tc0 = ((warp * G.T + t) * 8 + nt) * 4;
 #endif
             LSTM_STAMP(tc0);
-            // cell states of units nt * 32 + 2 i + q / 2 (cells 4 k .. 4 k + 3 in one float4), in flight during the k-loop
-            float4 *cp = cl + nt * (QN / 32) * 256;
-            float c_prev[QN / 8];
-#pragma unroll
-            for (int k = 0; k < QN / 32; k++) {
-                const float4 v = valid ? __ldcg(cp + k * 256) : make_float4(0.f, 0.f, 0.f, 0.f);
-                c_prev[4 * k] = v.x; c_prev[4 * k + 1] = v.y; c_prev[4 * k + 2] = v.z; c_prev[4 * k + 3] = v.w;
-            }
 #pragma unroll
             for (int i = 0; i < 64; i++) { hh[i] = 0; mix[i] = 0; }
             for (int kt = 0; kt < nkt; kt++, g++) {
-                const uint32_t s = g % QSTAGES, ph = (g / QSTAGES) & 1u;
+                const uint32_t s = g % LQSTAGES, ph = (g / LQSTAGES) & 1u;
                 mbar_wait(bar_full + 8 * s, ph);
                 if (kt == 0) LSTM_STAMP(tc0 + 1);
                 const uint32_t st = smem_base + s * QSTAGE_BYTES, a = st + (uint32_t) wg * 1024, b = st + 2 * QTILE_BYTES;
@@ -1041,60 +1159,29 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) k_lstm_layer_q8(LstmLayerQ G)
                 wg_wait<1>();
                 if (kt > 0) {
                     __syncwarp();
-                    if (lane == 0) mbar_arrive(bar_empty + 8 * ((g - 1) % QSTAGES));
+                    if (lane == 0) mbar_arrive(bar_empty + 8 * ((g - 1) % LQSTAGES));
                 }
             }
             wg_wait<0>();
             LSTM_STAMP(tc0 + 2);
             __syncwarp();
-            if (lane == 0) mbar_arrive(bar_empty + 8 * ((g - 1) % QSTAGES));
+            if (lane == 0) mbar_arrive(bar_empty + 8 * ((g - 1) % LQSTAGES));
 
             const float *sb = sbias + nt * QN + 2 * q, *ss = sscale + nt * QN + 2 * q;
-            // units nt * 32 .. + 31: slice k-tile 4 dir + nt / 2 (chunks 2 (nt & 1), + 1).  The even-unit lane writes slice 1
-            // of a unit pair, the odd-unit lane slice 0.
-            int8_t *qw = (odd_u ? G.q0 : G.q1) + mt * G.q_mt_stride + (int64_t) (tt * 8 + dir * 4 + (nt >> 1)) * QTILE_BYTES +
-                         (nt & 1) * 2 * 2048 + r128 * 16;
-            float *yf = G.y_f32 ? G.y_f32 + (int64_t) row * G.ldy + (int64_t) tt * 512 + dir * 256 + nt * (QN / 4) : nullptr;
+            if (n > 0) named_sync(LQ_FREE, LQ_HANDOFF_THREADS);       // the epilogue warps have read tile n - 1
 #pragma unroll
-            for (int m = 0; m < QN / 16; m++) {
-                int uq[4];
+            for (int i = 0; i < QN / 8; i++) {
+                const float2 bz = *reinterpret_cast<const float2 *>(sb + 8 * i), sz = *reinterpret_cast<const float2 *>(ss + 8 * i);
 #pragma unroll
-                for (int e = 0; e < 2; e++) {
-                    const int i = 2 * m + e;
-                    // gate columns 8 i + 2 q + {0, 1} of rows rA, rA + 8 (accumulator fragment of gates4)
-                    const float2 bz = *reinterpret_cast<const float2 *>(sb + 8 * i), sz = *reinterpret_cast<const float2 *>(ss + 8 * i);
-                    float v[4];
-#pragma unroll
-                    for (int k = 0; k < 4; k++)
-                        v[k] = fmaf(fmaf((float) hh[4 * i + k], 256.f, (float) mix[4 * i + k]), (k & 1) ? sz.y : sz.x, (k & 1) ? bz.y : bz.x);
-                    const float r0 = __shfl_xor_sync(0xffffffffu, (q & 1) ? v[0] : v[2], 1);
-                    const float r1 = __shfl_xor_sync(0xffffffffu, (q & 1) ? v[1] : v[3], 1);
-                    const float gi = (q & 1) ? r0 : v[0], gf = (q & 1) ? r1 : v[1];
-                    const float gg = (q & 1) ? v[2] : r0, go = (q & 1) ? v[3] : r1;
-                    const float cn = sigm(gf) * c_prev[i] + sigm(gi) * tanh_fast(gg);
-                    const float hn = sigm(go) * tanh_fast(cn);
-                    c_prev[i] = cn;
-                    const float hp = __shfl_xor_sync(0xffffffffu, hn, 2);
-                    const float h0 = odd_u ? hp : hn, h1 = odd_u ? hn : hp;          // units 2 i, 2 i + 1
-                    uq[2 * e] = qbias(h0); uq[2 * e + 1] = qbias(h1);
-                    if (yf && valid && !odd_u) *reinterpret_cast<float2 *>(yf + 2 * i) = make_float2(h0, h1);
-                }
-                // units nt * 32 + 4 m .. + 3 of row r128
-                if (valid) __stwb(reinterpret_cast<uint32_t *>(qw + (m >> 2) * 2048 + 4 * (m & 3)), qword(uq[0], uq[1], uq[2], uq[3], odd_u));
-                // cells 2 m - 2 .. 2 m + 1 are done: one 16 B store
-                if ((m & 1) && valid) {
-                    const int k = m >> 1;
-                    cp[k * 256] = make_float4(c_prev[4 * k], c_prev[4 * k + 1], c_prev[4 * k + 2], c_prev[4 * k + 3]);
+                for (int h = 0; h < 2; h++) {
+                    const float v0 = fmaf(fmaf((float) hh[4 * i + 2 * h], 256.f, (float) mix[4 * i + 2 * h]), sz.x, bz.x);
+                    const float v1 = fmaf(fmaf((float) hh[4 * i + 2 * h + 1], 256.f, (float) mix[4 * i + 2 * h + 1]), sz.y, bz.y);
+                    *reinterpret_cast<float2 *>(sp + i * 1024 + h * 32) = make_float2(v0, v1);
                 }
             }
             LSTM_STAMP(tc0 + 3);
+            named_arrive(LQ_STAGED, LQ_HANDOFF_THREADS);
         }
-        // h_t of this warp's rows is complete (all eight gate tiles): publish it to the producer thread
-        __threadfence();
-        LSTM_STAMP(256 * G.T + (warp * G.T + t) * 2);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_h);
-        LSTM_STAMP(256 * G.T + (warp * G.T + t) * 2 + 1);
     }
 #ifdef PB_LSTM_TRACE
     if (tr && threadIdx.x == 0) { tr[275 * G.T + 2] = trace_gtime(); tr[275 * G.T + 3] = trace_clock(); }
@@ -1140,7 +1227,7 @@ __global__ void __launch_bounds__(PG_THREADS, 1) k_gemm_q8(GemmQ G) {
                 const int64_t aoff = (int64_t) mt * G.a_mt_stride, woff = (int64_t) nt * G.nkt * QTILE_BYTES;
                 for (int kt = 0; kt < G.nkt; kt++, g++) {
                     const int64_t ko = (int64_t) kt * QTILE_BYTES;
-                    load_stage_q(smem_base, bar_full, bar_empty, g, G.a1 + aoff + ko, G.a0 + aoff + ko, G.w1 + woff + ko, G.w0 + woff + ko);
+                    load_stage_q<QSTAGES>(smem_base, bar_full, bar_empty, g, G.a1 + aoff + ko, G.a0 + aoff + ko, G.w1 + woff + ko, G.w0 + woff + ko);
                 }
             }
         }

@@ -2,12 +2,13 @@
 both variant LSTM layers of one VariantNet.predict chunk at each size (the encoder's k_lstm_layer_enc, or k_lstm_layer when
 its h-part runs all three products, and the decoder's k_lstm_layer_q8, or k_lstm_layer in mode 1).
 
-    python scripts/trace_lstm_layer.py [--sizes 8448 1408] [--lib TRACED.so] [--build-dir DIR] [--out FILE]
+    python scripts/trace_lstm_layer.py [--sizes 8448 1408] [--lib TRACED.so] [--build-dir DIR] [--out FILE] [--raw FILE.npz]
 
 Without --lib the traced library is built with `make EXTRA=-DPB_LSTM_TRACE` into --build-dir (default: a new temporary
 directory), never into the tree.  CTAs 0, n/2 and n-1 are sampled; every phase is the median (and mean) over those CTAs,
 their 8 consumer warps, steps 1..32 and the gate tiles, 4 in k_lstm_layer and 8 in k_lstm_layer_q8, or the 8 half gate tiles
-of k_lstm_layer_enc (producer phases: over CTAs and steps).  Times are SM cycles; the
+of k_lstm_layer_enc (producer phases: over CTAs and steps; k_lstm_layer_q8's epilogue warpgroup: over its 4 warps).  The
+hand-off rows of k_lstm_layer_q8 compare stamps of different warps of one SM (one %clock64).  Times are SM cycles; the
 kernel's own clock (cycles over %globaltimer) is printed beside the card name, power limit and nvidia-smi's SM clock.
 """
 import argparse
@@ -23,7 +24,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 T = 33                  # PB_VARIANT_WINDOW: steps per layer
 CTAS = 3                # LSTM_TRACE_CTAS
-CTA_WORDS = 275 * T + 4  # lstm_trace_cta_words(T)
+CTA_WORDS = 403 * T + 4  # lstm_trace_cta_words(T)
 
 
 def build_traced(build_dir: str) -> str:
@@ -64,7 +65,30 @@ def phases(words: np.ndarray) -> dict:
             tile = tile[:, :, :4]
         step = w[256 * T:272 * T].reshape(8, T, 2)         # [warp][t][fence returned, bar_h arrived]
         prod = w[272 * T:275 * T].reshape(T, 3)            # [t][bar_h wait start, wait end, first h copy issued]
+        epi = w[275 * T + 4:403 * T + 4].reshape(4, T, 8, 4)  # [epilogue warp][t][nt][staged wait, cells done, h published, -]
         tl = tile[:, 1:]
+        if epi.any():
+            # k_lstm_layer_q8: consumers [start, first full, wg_wait<0>, staging stored]; the epilogue warpgroup runs the
+            # cells of tile nt from the staging buffer under the k-loop of tile nt + 1.  "staged" is released when the last
+            # consumer warp has stored (bar.sync defers its blocking, so the epilogue warps have no stamp of the release).
+            el = epi[:, 1:]
+            stored = tile[:, 1:, :, 3].max(axis=0)           # [t][nt] the last consumer warp's staging stored
+            add("tile: start -> first bar_full", tl[..., 1] - tl[..., 0])
+            add("tile: first bar_full -> wg_wait<0> (k-loop)", tl[..., 2] - tl[..., 1])
+            add("tile: wg_wait<0> -> staging stored (hand-off)", tl[..., 3] - tl[..., 2])
+            add("tile: staging stored -> next tile start", tl[:, :, 1:, 0] - tl[:, :, :-1, 3])
+            add("tile period (start -> next start, same step)", tl[:, :, 1:, 0] - tl[:, :, :-1, 0])
+            add("step period (tile 0 start -> next tile 0 start)", tile[:, 2:, 0, 0] - tile[:, 1:-1, 0, 0])
+            add("epilogue: last consumer stored -> cells done", el[..., 1] - stored[None])
+            add("epilogue: cells done -> next tile's staging stored (slack)", stored[None, :, 1:] - el[:, :, :-1, 1])
+            add("step: tile 7 staged -> h published", el[:, :, 7, 2] - stored[None, :, 7])
+            add("step: h published (last warp) -> producer bar_h passed", prod[2:, 1] - epi[:, 1:-1, 7, 2].max(axis=0))
+            add("step: h published (last warp) -> next step's tile 0 k-loop end",
+                tile[:, 2:, 0, 2].max(axis=0) - epi[:, 1:-1, 7, 2].max(axis=0))
+            add("producer: bar_h wait", prod[1:, 1] - prod[1:, 0])
+            add("producer: bar_h passed -> first h copy issued", prod[1:, 2] - prod[1:, 1])
+            add("kernel (globaltimer, ns)", [meta[2] - meta[0]])
+            continue
         if not prod.any():
             # k_lstm_layer_enc (no bar_h): per half tile [start, first full, last k-tile issued, end], the previous half's
             # epilogue running between the k-tiles; per step [half 7's epilogue done, h published (named barrier passed)]
@@ -100,6 +124,7 @@ def main():
     ap.add_argument("--lib", default=None, help="an existing PB_LSTM_TRACE build of libpepper_b200.so")
     ap.add_argument("--build-dir", default=None, help="where to build the traced library (default: a temporary directory)")
     ap.add_argument("--out", default=None, help="write the result as JSON here")
+    ap.add_argument("--raw", default=None, help="write every size's stamps (both layers, uint64) as arrays of one .npz here")
     args = ap.parse_args()
     if any(n < 1 or n > 8448 for n in args.sizes):
         ap.error("--sizes must lie in 1..8448 (one network chunk)")
@@ -130,11 +155,13 @@ def main():
     rng = np.random.default_rng(0)
     res = {"lib": lib_path, "gpu_before": gpu_info(), "sizes": []}
     words = np.zeros(2 * CTAS * CTA_WORDS, dtype=np.uint64)
+    raw = {}
     for n in args.sizes:
         x = rng.integers(-30, 31, size=(n, T, 26), dtype=np.int8)
         for _ in range(3):                                # warm-up; the trace holds the last call
             net.predict(x)
         _lib.check(L.pb_lstm_trace_copy(words.ctypes.data_as(C.c_void_p), C.c_int64(words.size)), "pb_lstm_trace_copy")
+        raw[f"n{n}"] = words.copy()
         res["sizes"].append({"candidates": n, "ctas": 2 * ((n + 127) // 128),
                              "encoder": phases(words[:CTAS * CTA_WORDS]), "decoder": phases(words[CTAS * CTA_WORDS:])})
     res["gpu_after"] = gpu_info()
@@ -156,6 +183,8 @@ def main():
     if args.out:
         with open(args.out, "w") as f:
             json.dump(res, f, indent=1)
+    if args.raw:
+        np.savez(args.raw, **raw)
 
 
 if __name__ == "__main__":
